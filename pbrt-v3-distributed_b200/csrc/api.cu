@@ -753,6 +753,7 @@ static int trace_dev(b200pt_scene *s, uint64_t rays_dev, uint64_t out_dev, int64
     a.ray_o = reinterpret_cast<const float4 *>(rays_dev);
     a.ray_d = reinterpret_cast<const float4 *>(rays_dev) + 1;
     a.stride = 2;
+    a.out_stride = (int)sizeof(uint8_t);  // occ_out: one byte per ray (closest hits go to full_out)
     a.t_max_from_w = 1;
     a.count = s->d_work + 1;
     a.work = s->d_work;
@@ -1125,9 +1126,9 @@ int b200pt_render_create(b200pt_scene *scene, const b200pt_camera_desc *cam, con
     }
 
     // batch sizing: whole tiles, about B200PT_BATCH_PATHS path slots
-    // path slots per batch: ~200 B each, plus 5 x 60 floats with a SampledSpectrum host (16 Mi slots = 23 GB there, which
-    // fits the H100's 80 GB; smaller batches leave the traversal launches too few rays to keep the SMs busy)
-    size_t target = 16u << 20;
+    // path slots per batch: 256 B of records + ~40 B of queues each, plus 5 x 60 floats with a SampledSpectrum host.
+    // Larger batches keep the traversal launches fuller: RGB takes 32 Mi slots (~10 GB); 60 bins keep 16 Mi (~25 GB).
+    size_t target = scene->nspec ? (16u << 20) : (32u << 20);
     if (const char *e = getenv("B200PT_BATCH_PATHS")) target = (size_t)atoll(e);
     const size_t per_tile = 256u * (size_t)r->spp;
     r->tiles_per_batch = (uint32_t)std::max<size_t>(1, target / per_tile);
@@ -1161,22 +1162,8 @@ int b200pt_render_create(b200pt_scene *scene, const b200pt_camera_desc *cam, con
     ALLOC(H.sp_cdf, (size_t)nvox * (nl + 1));
     ALLOC(H.sp_func_int, (size_t)nvox);
     ALLOC(H.film, (size_t)cw * chh);
-    ALLOC(H.ray_o, cap);
-    ALLOC(H.ray_d, cap);
-    ALLOC(H.beta, cap);
-    ALLOC(H.L, cap);
-    ALLOC(H.sobol, cap);
-    ALLOC(H.hit, cap);
-    if (!scene->instances.empty()) ALLOC(H.hit_inst, cap);
-    ALLOC(H.sh_o, cap);
-    ALLOC(H.sh_d, cap);
-    ALLOC(H.A, cap);
-    ALLOC(H.mi_o, cap);
-    ALLOC(H.mi_d, cap);
-    ALLOC(H.B, cap);
-    ALLOC(H.beta_ld, cap);
-    ALLOC(H.occluded, cap);
-    ALLOC(H.mis_hit, cap);
+    ALLOC(H.path, cap);
+    ALLOC(H.direct, cap);
     ALLOC(H.pix_bleed, (size_t)r->tiles_per_batch * 256);
     float *d_light_spectra = nullptr;
     if (scene->nspec) {
@@ -1491,7 +1478,7 @@ int b200pt_render_tiles(b200pt_render *r, const int32_t *tiles, int64_t n_tiles)
                 a.n_instances = H.scene.n_instances;
                 a.tlas_node_off = H.scene.tlas_node_off;
                 a.tlas_tri_off = H.scene.tlas_tri_off;
-                a.hit_inst_out = a.hit_out == H.hit ? H.hit_inst : nullptr;
+                a.hit_inst_out = a.hit_out == &H.path->hit ? &H.path->hit_inst : nullptr;
                 launch_trace2(a, any_hit, classify, r->grid_trace, s_);
                 return;
             }
@@ -1506,7 +1493,7 @@ int b200pt_render_tiles(b200pt_render *r, const int32_t *tiles, int64_t n_tiles)
             a.n_instances = tl ? 0u : H.scene.n_instances;
             a.tlas_node_off = H.scene.tlas_node_off;
             a.tlas_tri_off = H.scene.tlas_tri_off;
-            a.hit_inst_out = a.hit_out == H.hit ? H.hit_inst : nullptr;
+            a.hit_inst_out = a.hit_out == &H.path->hit ? &H.path->hit_inst : nullptr;
             a.n_tris = (uint32_t)r->scene->n_prims;
             a.sphere_work = work;
         };
@@ -1518,7 +1505,8 @@ int b200pt_render_tiles(b200pt_render *r, const int32_t *tiles, int64_t n_tiles)
             trace_args_scene(a, r->scene);
             a.materials = H.scene.materials;
             a.stats = H.stats;
-            a.stride = 1;
+            a.stride = REC_F4;
+            a.out_stride = (int)sizeof(PathRec);
             a.refill_lanes = r->refill_lanes;
             a.postpone_pct = r->postpone_pct;
             a.ctas = r->trace_ctas;
@@ -1527,15 +1515,15 @@ int b200pt_render_tiles(b200pt_render *r, const int32_t *tiles, int64_t n_tiles)
             const bool sorted = r->sort_from_bounce >= 0 && b >= r->sort_from_bounce;
             if (sorted) {
                 LaunchTimer lt(r, st, 2);
-                launch_sort_queue(r->d_dev, H, H.q_path[b & 1], qc + Q_PATH, H.ray_o, H.ray_d, r->grid_shade, st);
+                launch_sort_queue(r->d_dev, H, H.q_path[b & 1], qc + Q_PATH, &H.path->o, &H.path->d, r->grid_shade, st);
             }
-            a.ray_o = H.ray_o;
-            a.ray_d = H.ray_d;
+            a.ray_o = &H.path->o;
+            a.ray_d = &H.path->d;
             a.queue = sorted ? H.q_sorted : H.q_path[b & 1];
             a.count = qc + Q_PATH;
             a.work = wk + 0;
             a.fixed_t_max = INFINITY;
-            a.hit_out = H.hit;
+            a.hit_out = &H.path->hit;
             for (int m = 0; m < 4; ++m) a.q_mat[m] = H.q_mat[m];
             a.qcount_mat = qc + Q_MAT0;
             {
@@ -1593,14 +1581,15 @@ int b200pt_render_tiles(b200pt_render *r, const int32_t *tiles, int64_t n_tiles)
             trace_args_scene(a, r->scene);
             a.materials = H.scene.materials;
             a.stats = H.stats;
-            a.stride = 1;
+            a.stride = REC_F4;
             a.refill_lanes = r->refill_lanes;
             a.postpone_pct = r->postpone_pct;
             a.ctas = r->trace_ctas;
-            a.ray_o = shadow ? H.sh_o : H.mi_o;
-            a.ray_d = shadow ? H.sh_d : H.mi_d;
+            a.ray_o = shadow ? &H.direct->sh_o : &H.direct->mi_o;
+            a.ray_d = shadow ? &H.direct->sh_d : &H.direct->mi_d;
             a.fixed_t_max = shadow ? PT_SHADOW_TMAX : INFINITY;
-            a.hit_out = shadow ? H.sh_hit : H.mis_hit;
+            a.hit_out = shadow ? H.sh_hit : &H.direct->mis_hit;
+            a.out_stride = shadow ? (int)sizeof(uint32_t) : (int)sizeof(DirectRec);
             const uint32_t *queue = shadow ? H.q_shadow : H.q_mis;
             const uint32_t *count = qc + (shadow ? Q_SHADOW : Q_MIS);
             uint32_t *trace_work = wk + (shadow ? 5 : 6), *sphere_work = wk + (shadow ? 9 : 10);
@@ -1646,7 +1635,8 @@ int b200pt_render_tiles(b200pt_render *r, const int32_t *tiles, int64_t n_tiles)
             trace_args_scene(a, r->scene);
             a.materials = H.scene.materials;
             a.stats = H.stats;
-            a.stride = 1;
+            a.stride = REC_F4;
+            a.out_stride = (int)sizeof(DirectRec);
             a.refill_lanes = r->refill_lanes;
             a.postpone_pct = r->postpone_pct;
             a.ctas = r->trace_ctas;
@@ -1655,15 +1645,15 @@ int b200pt_render_tiles(b200pt_render *r, const int32_t *tiles, int64_t n_tiles)
             const bool sorted_sh = r->sort_from_bounce >= 0;
             if (sorted_sh) {
                 LaunchTimer lt(r, st2, 2);
-                launch_sort_queue(r->d_dev, H, H.q_shadow, qc + Q_SHADOW, H.sh_o, H.sh_d, r->grid_shade, st2);
+                launch_sort_queue(r->d_dev, H, H.q_shadow, qc + Q_SHADOW, &H.direct->sh_o, &H.direct->sh_d, r->grid_shade, st2);
             }
-            a.ray_o = H.sh_o;
-            a.ray_d = H.sh_d;
+            a.ray_o = &H.direct->sh_o;
+            a.ray_d = &H.direct->sh_d;
             a.queue = sorted_sh ? H.q_sorted : H.q_shadow;
             a.count = qc + Q_SHADOW;
             a.work = wk + 5;
             a.fixed_t_max = PT_SHADOW_TMAX;
-            a.occ_out = H.occluded;
+            a.occ_out = &H.direct->occluded;
             {
                 LaunchTimer lt(r, st2, 1);
                 trace(a, true, false, st2);
@@ -1674,13 +1664,13 @@ int b200pt_render_tiles(b200pt_render *r, const int32_t *tiles, int64_t n_tiles)
                 }
             }
             // BSDF-sampled MIS rays (closest hit)
-            a.ray_o = H.mi_o;
-            a.ray_d = H.mi_d;
+            a.ray_o = &H.direct->mi_o;
+            a.ray_d = &H.direct->mi_d;
             a.queue = H.q_mis;
             a.count = qc + Q_MIS;
             a.work = wk + 6;
             a.fixed_t_max = INFINITY;
-            a.hit_out = H.mis_hit;
+            a.hit_out = &H.direct->mis_hit;
             a.occ_out = nullptr;
             LaunchTimer lt(r, st2, 0);
             trace(a, false, false, st2);
@@ -1947,9 +1937,9 @@ int b200pt_debug_pixel_samples(b200pt_render *r, int32_t px, int32_t py, float *
     if (rc == B200PT_OK) {
         const uint32_t pix = (uint32_t)((py - (H.sampler.sb[1] + ty * 16)) * 16 + (px - (H.sampler.sb[0] + tx * 16)));
         const int ns = r->scene->nspec;
-        std::vector<float4> tmp((size_t)r->spp);
+        std::vector<PathRec> tmp((size_t)r->spp);
         std::vector<float> bins((size_t)r->spp * (size_t)std::max(ns, 1));
-        cudaError_t e = cudaMemcpyAsync(tmp.data(), H.L + (size_t)pix * r->spp, (size_t)r->spp * sizeof(float4),
+        cudaError_t e = cudaMemcpyAsync(tmp.data(), H.path + (size_t)pix * r->spp, (size_t)r->spp * sizeof(PathRec),
                                         cudaMemcpyDeviceToHost, st);
         if (ns && e == cudaSuccess)  // slot-major [capacity][bins]: the pixel's samples are consecutive slots
             e = cudaMemcpyAsync(bins.data(), H.s_L + (size_t)pix * r->spp * ns, (size_t)r->spp * ns * sizeof(float),
@@ -1959,7 +1949,7 @@ int b200pt_debug_pixel_samples(b200pt_render *r, int32_t px, int32_t py, float *
         if (e != cudaSuccess) rc = b200pt_fail(B200PT_ERR_CUDA, "debug_pixel_samples: %s", cudaGetErrorString(e));
         for (int i = 0; i < r->spp && rc == B200PT_OK; ++i) {
             if (!ns) {
-                Spec L = rgb(tmp[i].x, tmp[i].y, tmp[i].z);
+                Spec L = rgb(tmp[i].L.x, tmp[i].L.y, tmp[i].L.z);
                 if (has_nans(L) || lum(L) < -1e-5f || pt_isinf(lum(L))) L = rgb1(0.f);  // integrator.cpp:294-315
                 out_rgb[3 * i] = L.c[0];
                 out_rgb[3 * i + 1] = L.c[1];

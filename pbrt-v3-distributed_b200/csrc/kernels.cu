@@ -21,19 +21,17 @@ namespace B200PT_NS {
 __device__ __forceinline__ V3 v3(const float4 &f) { return mk(f.x, f.y, f.z); }
 __device__ __forceinline__ V3 v3(const F4 &f) { return mk(f.x, f.y, f.z); }
 __device__ __forceinline__ float4 f4(const V3 &v, float w) { return make_float4(v.x, v.y, v.z, w); }
-// A per-slot spectrum travels with one packed scalar.  RGBSpectrum build: one float4 (r, g, b, w).  SampledSpectrum
-// build: the float4 keeps only w and the 60 bins live slot-major in a second array, [capacity][60] (240 contiguous bytes
-// per slot, read and written as float4s).  A [bin][capacity] layout would coalesce only if a warp's slots were neighbours;
-// the slots of a BSDF family's queue are scattered, so every 4-byte access would cost a 32-byte sector of DRAM traffic.
-__device__ __forceinline__ Spec ld_spec(const float4 *a4, const float *bins, uint32_t cap, uint32_t slot, float *w) {
-    const float4 f = a4[slot];
+// A per-slot spectrum travels with one packed scalar.  RGBSpectrum build: one float4 of a record (r, g, b, w).
+// SampledSpectrum build: the float4 keeps only w and the 60 bins live slot-major in a second array, [capacity][60] (240
+// contiguous bytes per slot, read and written as float4s).  A [bin][capacity] layout would coalesce only if a warp's slots
+// were neighbours; the slots of a BSDF family's queue are scattered, so every 4-byte access would cost a 32-byte sector.
+__device__ __forceinline__ Spec ld_spec(const float4 &f, const float *bins, uint32_t slot, float *w) {
     *w = f.w;
 #if B200PT_NSPEC == 3
     (void)bins;
-    (void)cap;
+    (void)slot;
     return rgb(f.x, f.y, f.z);
 #else
-    (void)cap;
     Spec s;
     const float4 *p4 = reinterpret_cast<const float4 *>(bins + (size_t)slot * B200PT_NSPEC);
 #pragma unroll
@@ -47,18 +45,26 @@ __device__ __forceinline__ Spec ld_spec(const float4 *a4, const float *bins, uin
     return s;
 #endif
 }
-__device__ __forceinline__ void st_spec(float4 *a4, float *bins, uint32_t cap, uint32_t slot, const Spec &s, float w) {
+__device__ __forceinline__ void st_spec(float4 &f, float *bins, uint32_t slot, const Spec &s, float w) {
 #if B200PT_NSPEC == 3
     (void)bins;
-    (void)cap;
-    a4[slot] = make_float4(s.c[0], s.c[1], s.c[2], w);
+    (void)slot;
+    f = make_float4(s.c[0], s.c[1], s.c[2], w);
 #else
-    (void)cap;
-    a4[slot] = make_float4(0.f, 0.f, 0.f, w);
+    f = make_float4(0.f, 0.f, 0.f, w);
     float4 *p4 = reinterpret_cast<float4 *>(bins + (size_t)slot * B200PT_NSPEC);
 #pragma unroll
     for (int q = 0; q < B200PT_NSPEC / 4; ++q) p4[q] = make_float4(s.c[4 * q], s.c[4 * q + 1], s.c[4 * q + 2], s.c[4 * q + 3]);
 #endif
+}
+// Shading writes beta_ld's sector whole: the traversal results beside it are reset with one 16-byte store (the shadow and
+// MIS launches of the bounce overwrite them before anything reads them).
+__device__ __forceinline__ void reset_direct_hits(DirectRec &D) {
+    *reinterpret_cast<float4 *>(&D.mis_hit) = make_float4(__uint_as_float(B200PT_MISS), 0.f, 0.f, 0.f);
+}
+__device__ __forceinline__ void st_beta_ld(DirectRec &D, float *bins, uint32_t slot, const Spec &beta, float pickPdf) {
+    st_spec(D.beta_ld, bins, slot, beta, pickPdf);
+    reset_direct_hits(D);
 }
 // Lemit / I / L of light `lightNum` (b200pt_area_light::lemit, or its row of b200pt_scene_desc::light_spectra)
 __device__ __forceinline__ Spec light_emit(const RenderDev *R, int lightNum, const DevLight &l) {
@@ -207,12 +213,15 @@ __global__ void __launch_bounds__(256) k_raygen(const RenderDev *R, uint32_t fir
             if ((int)floorf(dy + 0.5f) + 1 > py + 1) code |= 8u;
             if (code) R->pix_bleed[tb * 256u + pix] = 1;
             if (R->filter_general) R->pfilm[slot] = make_float2(pFilm[0], pFilm[1]);
-            R->sobol[slot] = st.index;
-            R->ray_o[slot] = f4(o, 1.f);                                // etaScale = 1
-            R->ray_d[slot] = f4(d, __uint_as_float((uint32_t)st.dim));  // dim = 5, bounces = 0, flags = 0
-            st_spec(R->beta, R->s_beta, R->capacity, slot, rgb1(1.f), 0.f);
-            st_spec(R->L, R->s_L, R->capacity, slot, rgb1(0.f), __uint_as_float(code));
-            R->sh_d[slot] = make_float4(0.f, 0.f, 0.f, 0.f);
+            PathRec &P = R->path[slot];
+            P.o = f4(o, 1.f);                                // etaScale = 1
+            P.d = f4(d, __uint_as_float((uint32_t)st.dim));  // dim = 5, bounces = 0, flags = 0
+            st_spec(P.beta, R->s_beta, slot, rgb1(1.f), 0.f);
+            st_spec(P.L, R->s_L, slot, rgb1(0.f), __uint_as_float(code));
+            P.sobol = st.index;
+            DirectRec &D = R->direct[slot];  // no direct lighting pending
+            D.sh_o = make_float4(0.f, 0.f, 0.f, 0.f);
+            D.sh_d = make_float4(0.f, 0.f, 0.f, 0.f);
             if (R->med_general) R->cur_med[slot] = R->has_medium ? 0 : -1;  // the camera's medium (camera.h:76)
         }
     }
@@ -257,10 +266,10 @@ void k_trace(const TraceArgs a) {
         const uint32_t best = traverse_wbvh<ANY_HIT, COUNT>(a.nodes, a.tri_base, a.tris, a.bounds, a.lut, v3(o4), v3(d4),
                                                             a.t_max_from_w ? o4.w : a.fixed_t_max, &hit, &ctr, &overflow);
         if (ANY_HIT) {
-            a.occ_out[slot] = best != B200PT_MISS ? 1 : 0;
+            slot_out(a.occ_out, slot, a.out_stride) = best != B200PT_MISS ? 1 : 0;
             continue;
         }
-        if (a.hit_out) a.hit_out[slot] = best;
+        if (a.hit_out) slot_out(a.hit_out, slot, a.out_stride) = best;
         if (a.full_out) {
             b200pt_hit r;
             r.triangle = best != B200PT_MISS ? (int32_t)__float_as_uint(ld_f4(a.tris + (size_t)best * 3).w) : -1;
@@ -456,9 +465,9 @@ __global__ void __launch_bounds__(128, CTAS) k_trace(const TraceArgs a) {
             if (fin) {
                 const uint32_t best = __float_as_uint(my_ray[8 * 128]);
                 if (ANY_HIT) {
-                    a.occ_out[slot] = best != B200PT_MISS ? 1 : 0;
+                    slot_out(a.occ_out, slot, a.out_stride) = best != B200PT_MISS ? 1 : 0;
                 } else {
-                    if (a.hit_out) a.hit_out[slot] = best;
+                    if (a.hit_out) slot_out(a.hit_out, slot, a.out_stride) = best;
                     if (a.full_out) {
                         b200pt_hit r;
                         r.triangle = best != B200PT_MISS ? (int32_t)__float_as_uint(ld_f4(a.tris + (size_t)best * 3).w) : -1;
@@ -761,10 +770,10 @@ __global__ void __launch_bounds__(128, 6) k_trace2(const TraceArgs a) {
             if (fin) {
                 const uint32_t best = __float_as_uint(my_ray[8 * 128]);
                 if (ANY_HIT) {
-                    a.occ_out[slot] = best != B200PT_MISS ? 1 : 0;
+                    slot_out(a.occ_out, slot, a.out_stride) = best != B200PT_MISS ? 1 : 0;
                 } else {
-                    if (a.hit_out) a.hit_out[slot] = best;
-                    if (a.hit_inst_out && best != B200PT_MISS) a.hit_inst_out[slot] = __float_as_uint(my_ray[21 * 128]);
+                    if (a.hit_out) slot_out(a.hit_out, slot, a.out_stride) = best;
+                    if (a.hit_inst_out && best != B200PT_MISS) slot_out(a.hit_inst_out, slot, a.out_stride) = __float_as_uint(my_ray[21 * 128]);
                     if (a.full_out) {
                         b200pt_hit r;
                         r.triangle = best != B200PT_MISS ? (int32_t)__float_as_uint(ld_f4(a.tris + (size_t)best * 3).w) : -1;
@@ -1135,12 +1144,12 @@ __global__ void __launch_bounds__(128) k_spheres(const TraceArgs a) {
             int family = -1;
             if (fin) {
                 if (ANY_HIT) {
-                    if (occluded || W.best != B200PT_MISS) a.occ_out[slot] = 1;
+                    if (occluded || W.best != B200PT_MISS) slot_out(a.occ_out, slot, a.out_stride) = 1;
                 } else {
                     if (W.best != B200PT_MISS) {
                         best = W.best;
-                        if (a.hit_out) a.hit_out[slot] = best;
-                        if (a.hit_inst_out) a.hit_inst_out[slot] = W.inst;
+                        if (a.hit_out) slot_out(a.hit_out, slot, a.out_stride) = best;
+                        if (a.hit_inst_out) slot_out(a.hit_inst_out, slot, a.out_stride) = W.inst;
                         if (a.full_out) {
                             b200pt_hit r;
                             r.triangle = (int32_t)__float_as_uint(ld_f4(a.tris + (size_t)best * 3).w);
@@ -1201,17 +1210,17 @@ __global__ void __launch_bounds__(128) k_spheres(const TraceArgs a) {
                 best = B200PT_MISS;
                 occluded = false;
                 if (ANY_HIT) {
-                    occluded = a.occ_out[slot] != 0;
+                    occluded = slot_out(a.occ_out, slot, a.out_stride) != 0;
                     for (uint32_t k = 0; k < a.n_spheres && !occluded; ++k) {
                         float t;
                         if (sphere_leaf_test(a.spheres[k], ro, rd, tmax) && sphere_intersect(a.spheres[k], ro, rd, tmax, &t, nullptr)) {
-                            a.occ_out[slot] = 1;
+                            slot_out(a.occ_out, slot, a.out_stride) = 1;
                             occluded = true;
                         }
                     }
                 } else {
                     if (a.hit_out) {
-                        best = a.hit_out[slot];
+                        best = slot_out(a.hit_out, slot, a.out_stride);
                         if (best != B200PT_MISS) {  // ray.tMax after the triangle hit: Triangle::Intersect's t
                             const F4 *tp = a.tris + (size_t)best * 3;
                             const F4 t0 = ld_f4(tp), t1 = ld_f4(tp + 1), t2 = ld_f4(tp + 2);
@@ -1220,7 +1229,7 @@ __global__ void __launch_bounds__(128) k_spheres(const TraceArgs a) {
                                 // a triangle of an instanced object (found by the two-level kernel): the same ray parameter in
                                 // the object's space (primitive.cpp:91)
                                 float tm2;
-                                instance_ray(a.instances[a.hit_inst_out[slot]], ro, rd, pt_inf(), &o2, &d2, &tm2);
+                                instance_ray(a.instances[slot_out(a.hit_inst_out, slot, a.out_stride)], ro, rd, pt_inf(), &o2, &d2, &tm2);
                             }
                             TriHit h;
                             if (triangle_test(v3(t0), v3(t1), v3(t2), o2, make_shear(d2), pt_inf(), &h)) tmax = h.t;
@@ -1239,7 +1248,7 @@ __global__ void __launch_bounds__(128) k_spheres(const TraceArgs a) {
                     }
                     if (sph != B200PT_MISS) {
                         best = SPHERE_HIT_BASE | sph;
-                        if (a.hit_out) a.hit_out[slot] = best;
+                        if (a.hit_out) slot_out(a.hit_out, slot, a.out_stride) = best;
                         if (a.full_out) {
                             b200pt_hit r;
                             r.triangle = (int32_t)(a.n_tris + sph);
@@ -1533,7 +1542,7 @@ __global__ void __launch_bounds__(128, B200PT_SHADE_MINCTAS) k_shade(const Rende
     bool have = warp_fetch(work, n, &i_next);
     if (have && i_next < n) {
         slot_next = queue[i_next];
-        hit_next = R->hit[slot_next];
+        hit_next = R->path[slot_next].hit;
     }
     while (have) {
         i = i_next;
@@ -1543,12 +1552,10 @@ __global__ void __launch_bounds__(128, B200PT_SHADE_MINCTAS) k_shade(const Rende
         hit_next = B200PT_MISS;
         if (have && i_next < n) {
             slot_next = queue[i_next];
-            asm volatile("prefetch.global.L2 [%0];" ::"l"(R->ray_o + slot_next));
-            asm volatile("prefetch.global.L2 [%0];" ::"l"(R->ray_d + slot_next));
-            asm volatile("prefetch.global.L2 [%0];" ::"l"(R->beta + slot_next));
-            asm volatile("prefetch.global.L2 [%0];" ::"l"(R->L + slot_next));
-            asm volatile("prefetch.global.L2 [%0];" ::"l"(R->sobol + slot_next));
-            hit_next = R->hit[slot_next];
+            asm volatile("prefetch.global.L2 [%0];" ::"l"(&R->path[slot_next].o));
+            asm volatile("prefetch.global.L2 [%0];" ::"l"(&R->path[slot_next].beta));
+            asm volatile("prefetch.global.L2 [%0];" ::"l"(&R->path[slot_next].sobol));
+            hit_next = R->path[slot_next].hit;
         }
 #else
     while (warp_fetch(work, n, &i)) {
@@ -1562,16 +1569,17 @@ __global__ void __launch_bounds__(128, B200PT_SHADE_MINCTAS) k_shade(const Rende
 #else
             slot = queue[i];
 #endif
-            const float4 o4 = R->ray_o[slot], d4 = R->ray_d[slot];
+            PathRec &P = R->path[slot];
+            const float4 o4 = P.o, d4 = P.d;
             float betaW, LW;
-            Spec beta = ld_spec(R->beta, R->s_beta, R->capacity, slot, &betaW);
-            Spec L = ld_spec(R->L, R->s_L, R->capacity, slot, &LW);
+            Spec beta = ld_spec(P.beta, R->s_beta, slot, &betaW);
+            Spec L = ld_spec(P.L, R->s_L, slot, &LW);
             const V3 ro = v3(o4), rd = v3(d4);
             float etaScale = o4.w;
             const uint32_t meta = __float_as_uint(d4.w);
             const int bounces = (int)((meta >> 16) & 0xffu);
             const bool specularBounce = ((meta >> 24) & PF_SPECULAR) != 0;
-            const uint32_t ti = R->hit[slot];
+            const uint32_t ti = P.hit;
             Isect is;
             uint32_t mflags;
             int lightId;
@@ -1593,7 +1601,7 @@ __global__ void __launch_bounds__(128, B200PT_SHADE_MINCTAS) k_shade(const Rende
                 TriHit h;
                 if (VTX && (mflags & 0x100000u)) {
                     // a triangle of an instanced object: intersect in the object's space, bring the hit back
-                    const DevInstance *in = R->scene.instances + R->hit_inst[slot];
+                    const DevInstance *in = R->scene.instances + P.hit_inst;
                     V3 o2, d2;
                     float tm2;
                     instance_ray(*in, ro, rd, pt_inf(), &o2, &d2, &tm2);
@@ -1627,7 +1635,7 @@ __global__ void __launch_bounds__(128, B200PT_SHADE_MINCTAS) k_shade(const Rende
                     const uint32_t mi = mflags & 0xffffu;
                     make_bsdf<MAT>(R->scene.materials[mi], R->scene.material_spectra + (size_t)mi * (5 * B200PT_NSPEC), is, &bsdf);
                     SobolStream st;
-                    st.index = R->sobol[slot];
+                    st.index = P.sobol;
                     st.dim = (int)(meta & 0xffffu);
                     st.px = st.py = 0;  // only dimensions 0/1 depend on the pixel
                     const SamplerParams &sp = R->sampler;
@@ -1652,18 +1660,21 @@ __global__ void __launch_bounds__(128, B200PT_SHADE_MINCTAS) k_shade(const Rende
                             const int med = (B200PT_MEDIA_GENERAL && VTX && R->med_general) ? R->cur_med[slot] : 0;
                             estimate_direct<VTX, mat_kinds(MAT)>(R, is, bsdf, uScattering, lightNum, uLight, &dout, false, med);
                             pend = dout.pend;
+                            // without pending rays nothing is stored: k_resolve left the pending flags at 0
                             if (pend) {
-                                st_spec(R->beta_ld, R->s_beta_ld, R->capacity, slot, beta, pickPdf);
-                                R->sh_o[slot] = f4(dout.sh_o, __uint_as_float((uint32_t)lightNum));
-                                if (pend & PEND_LIGHT) st_spec(R->A, R->s_A, R->capacity, slot, dout.A, dout.wA);
+                                DirectRec &D = R->direct[slot];
+                                D.sh_o = f4(dout.sh_o, __uint_as_float((uint32_t)lightNum));
+                                D.sh_d = f4(dout.sh_d, __uint_as_float(pend));
                                 if (pend & PEND_BSDF) {
-                                    R->mi_o[slot] = f4(dout.mi_o, dout.pdfB);
-                                    R->mi_d[slot] = f4(dout.mi_d, 0.f);
-                                    st_spec(R->B, R->s_B, R->capacity, slot, dout.B, dout.wB);
+                                    D.mi_o = f4(dout.mi_o, dout.pdfB);
+                                    D.mi_d = f4(dout.mi_d, 0.f);
                                 }
+                                // A and B share a sector: both are stored (the one not pending is never read)
+                                st_spec(D.A, R->s_A, slot, dout.A, dout.wA);
+                                st_spec(D.B, R->s_B, slot, dout.B, dout.wB);
+                                st_beta_ld(D, R->s_beta_ld, slot, beta, pickPdf);
                                 if (B200PT_MEDIA_GENERAL && VTX && R->med_general) store_direct_general(R, slot, dout, med);
                             }
-                            R->sh_d[slot] = f4(dout.sh_d, __uint_as_float(pend));
                         }
                     }
                     // path.cpp:131-150: sample the BSDF for the next direction
@@ -1695,13 +1706,15 @@ __global__ void __launch_bounds__(128, B200PT_SHADE_MINCTAS) k_shade(const Rende
                         if (cont) {
                             const uint32_t nmeta = ((uint32_t)st.dim & 0xffffu) | ((uint32_t)(bounces + 1) << 16) |
                                                    ((spec ? (uint32_t)PF_SPECULAR : 0u) << 24);
-                            R->ray_o[slot] = f4(no, etaScale);
-                            R->ray_d[slot] = f4(wi, __uint_as_float(nmeta));
-                            st_spec(R->beta, R->s_beta, R->capacity, slot, beta, 0.f);
+                            P.o = f4(no, etaScale);
+                            P.d = f4(wi, __uint_as_float(nmeta));
+                            betaW = 0.f;
                         }
                     }
                 }
-                st_spec(R->L, R->s_L, R->capacity, slot, L, LW);
+                // beta and L share a sector: both are stored (the beta of a path that ends here is never read)
+                st_spec(P.beta, R->s_beta, slot, beta, betaW);
+                st_spec(P.L, R->s_L, slot, L, LW);
             }
         }
         const uint32_t ps = warp_append(qc_shadow, (pend & PEND_LIGHT) != 0);
@@ -1999,7 +2012,7 @@ __global__ void __launch_bounds__(128, B200PT_S60_SHADE_MINCTAS) k_shade(const R
         uint32_t pend = 0, slot = 0;
         if (active) {
             slot = queue[i];
-            const float4 o4 = R->ray_o[slot], d4 = R->ray_d[slot];
+            const float4 o4 = R->path[slot].o, d4 = R->path[slot].d;
             float4 *sBeta = reinterpret_cast<float4 *>(R->s_beta + (size_t)slot * B200PT_NSPEC);
             float4 *sL = reinterpret_cast<float4 *>(R->s_L + (size_t)slot * B200PT_NSPEC);
             const V3 ro = v3(o4), rd = v3(d4);
@@ -2007,7 +2020,7 @@ __global__ void __launch_bounds__(128, B200PT_S60_SHADE_MINCTAS) k_shade(const R
             const uint32_t meta = __float_as_uint(d4.w);
             const int bounces = (int)((meta >> 16) & 0xffu);
             const bool specularBounce = ((meta >> 24) & PF_SPECULAR) != 0;
-            const uint32_t ti = R->hit[slot];
+            const uint32_t ti = R->path[slot].hit;
             Isect is;
             uint32_t mflags;
             int lightId;
@@ -2026,7 +2039,7 @@ __global__ void __launch_bounds__(128, B200PT_S60_SHADE_MINCTAS) k_shade(const R
                 lightId = (int)__float_as_uint(t2.w);
                 TriHit h;
                 if (mflags & 0x100000u) {
-                    const DevInstance *in = R->scene.instances + R->hit_inst[slot];
+                    const DevInstance *in = R->scene.instances + R->path[slot].hit_inst;
                     V3 o2, d2;
                     float tm2;
                     instance_ray(*in, ro, rd, pt_inf(), &o2, &d2, &tm2);
@@ -2067,7 +2080,7 @@ __global__ void __launch_bounds__(128, B200PT_S60_SHADE_MINCTAS) k_shade(const R
                     const uint32_t mi = mflags & 0xffffu;
                     make_bsdf<MAT>(R->scene.materials[mi], R->scene.material_spectra + (size_t)mi * (5 * B200PT_NSPEC), is, &bsdf);
                     SobolStream st;
-                    st.index = R->sobol[slot];
+                    st.index = R->path[slot].sobol;
                     st.dim = (int)(meta & 0xffffu);
                     st.px = st.py = 0;
                     const SamplerParams &sp = R->sampler;
@@ -2089,21 +2102,24 @@ __global__ void __launch_bounds__(128, B200PT_S60_SHADE_MINCTAS) k_shade(const R
                             DirectLazy dout;
                             estimate_direct_lazy<mat_kinds(MAT)>(R, slot, is, bsdf, uScattering, lightNum, uLight, &dout);
                             pend = dout.pend;
+                            // without pending rays nothing is stored: k_resolve left the pending flags at 0
                             if (pend) {
                                 // beta as it is before this vertex's BSDF sample scales it
                                 float4 *sBl = reinterpret_cast<float4 *>(R->s_beta_ld + (size_t)slot * B200PT_NSPEC);
 #pragma unroll 5
                                 for (int q = 0; q < B200PT_NSPEC / 4; ++q) sBl[q] = sBeta[q];
-                                R->beta_ld[slot] = make_float4(0.f, 0.f, 0.f, pickPdf);
-                                R->sh_o[slot] = f4(dout.sh_o, __uint_as_float((uint32_t)lightNum));
-                                if (pend & PEND_LIGHT) R->A[slot] = make_float4(0.f, 0.f, 0.f, 0.f);
+                                DirectRec &D = R->direct[slot];
+                                D.sh_o = f4(dout.sh_o, __uint_as_float((uint32_t)lightNum));
+                                D.sh_d = f4(dout.sh_d, __uint_as_float(pend));
                                 if (pend & PEND_BSDF) {
-                                    R->mi_o[slot] = f4(dout.mi_o, 0.f);
-                                    R->mi_d[slot] = f4(dout.mi_d, 0.f);
-                                    R->B[slot] = make_float4(0.f, 0.f, 0.f, 0.f);
+                                    D.mi_o = f4(dout.mi_o, 0.f);
+                                    D.mi_d = f4(dout.mi_d, 0.f);
                                 }
+                                D.A = make_float4(0.f, 0.f, 0.f, 0.f);
+                                D.B = make_float4(0.f, 0.f, 0.f, 0.f);
+                                D.beta_ld = make_float4(0.f, 0.f, 0.f, pickPdf);
+                                reset_direct_hits(D);
                             }
-                            R->sh_d[slot] = f4(dout.sh_d, __uint_as_float(pend));
                         }
                     }
                     // path.cpp:131-150
@@ -2157,9 +2173,9 @@ __global__ void __launch_bounds__(128, B200PT_S60_SHADE_MINCTAS) k_shade(const R
                         if (cont) {
                             const uint32_t nmeta = ((uint32_t)st.dim & 0xffffu) | ((uint32_t)(bounces + 1) << 16) |
                                                    ((spec ? (uint32_t)PF_SPECULAR : 0u) << 24);
-                            R->ray_o[slot] = f4(no, etaScale);
-                            R->ray_d[slot] = f4(wi, __uint_as_float(nmeta));
-                            R->beta[slot] = make_float4(0.f, 0.f, 0.f, 0.f);
+                            R->path[slot].o = f4(no, etaScale);
+                            R->path[slot].d = f4(wi, __uint_as_float(nmeta));
+                            R->path[slot].beta = make_float4(0.f, 0.f, 0.f, 0.f);
                         }
                     }
                 }
@@ -2203,12 +2219,12 @@ __global__ void __launch_bounds__(128, 4) k_medium(const RenderDev *R, int bounc
         uint32_t pend = 0, slot = 0;
         if (active) {
             slot = queue[i];
-            const float4 o4 = R->ray_o[slot], d4 = R->ray_d[slot];
+            const float4 o4 = R->path[slot].o, d4 = R->path[slot].d;
 #if B200PT_NSPEC == 3
             float betaW;
-            Spec beta = ld_spec(R->beta, R->s_beta, R->capacity, slot, &betaW);
+            Spec beta = ld_spec(R->path[slot].beta, R->s_beta, slot, &betaW);
 #else
-            const float betaW = R->beta[slot].w;
+            const float betaW = R->path[slot].beta.w;
             float4 *sBeta = reinterpret_cast<float4 *>(R->s_beta + (size_t)slot * B200PT_NSPEC);
 #endif
             const V3 ro = v3(o4), rd = v3(d4);
@@ -2216,7 +2232,7 @@ __global__ void __launch_bounds__(128, 4) k_medium(const RenderDev *R, int bounc
             const uint32_t meta = __float_as_uint(d4.w);
             const int bounces = (int)((meta >> 16) & 0xffu);
             // distance of the closest hit (ray.tMax after Scene::Intersect) and its material
-            const uint32_t ti = R->hit[slot];
+            const uint32_t ti = R->path[slot].hit;
             float tHit = pt_inf();
             uint32_t mflags = 0;
             if (ti != B200PT_MISS) {
@@ -2232,14 +2248,14 @@ __global__ void __launch_bounds__(128, 4) k_medium(const RenderDev *R, int bounc
                     V3 o2 = ro, d2 = rd;
                     if (mflags & 0x100000u) {  // a triangle of an instanced object: same ray parameter in the object's space
                         float tm2;
-                        instance_ray(R->scene.instances[R->hit_inst[slot]], ro, rd, pt_inf(), &o2, &d2, &tm2);
+                        instance_ray(R->scene.instances[R->path[slot].hit_inst], ro, rd, pt_inf(), &o2, &d2, &tm2);
                     }
                     TriHit h;
                     if (triangle_test(v3(t0), v3(t1), v3(t2), o2, make_shear(d2), pt_inf(), &h)) tHit = h.t;
                 }
             }
             SobolStream st;
-            st.index = R->sobol[slot];
+            st.index = R->path[slot].sobol;
             st.dim = (int)(meta & 0xffffu);
             st.px = st.py = 0;
             const SamplerParams &sp = R->sampler;
@@ -2290,11 +2306,11 @@ __global__ void __launch_bounds__(128, 4) k_medium(const RenderDev *R, int bounc
                 if (!sampledMedium) {
                     // on to the surface vertex (or out of the scene)
 #if B200PT_NSPEC == 3
-                    st_spec(R->beta, R->s_beta, R->capacity, slot, beta, betaW);
+                    st_spec(R->path[slot].beta, R->s_beta, slot, beta, betaW);
 #else
-                    R->beta[slot] = make_float4(0.f, 0.f, 0.f, betaW);
+                    R->path[slot].beta = make_float4(0.f, 0.f, 0.f, betaW);
 #endif
-                    R->ray_d[slot] = f4(rd, __uint_as_float((meta & 0xffff0000u) | ((uint32_t)st.dim & 0xffffu)));
+                    R->path[slot].d = f4(rd, __uint_as_float((meta & 0xffff0000u) | ((uint32_t)st.dim & 0xffffu)));
                     if (ti != B200PT_MISS) family = R->scene.materials[mflags & 0xffffu].type;
                 } else if (bounces < R->max_depth) {  // volpath.cpp:84-85
                     Isect mi;  // MediumInteraction(ray(t), -ray.d, ...): no normal, no error bounds
@@ -2325,13 +2341,13 @@ __global__ void __launch_bounds__(128, 4) k_medium(const RenderDev *R, int bounc
                             estimate_direct<true>(R, mi, none, uScattering, lightNum, uLight, &dout, true);
                             pend = dout.pend;
                             if (pend) {
-                                st_spec(R->beta_ld, R->s_beta_ld, R->capacity, slot, beta, pickPdf);
-                                R->sh_o[slot] = f4(dout.sh_o, __uint_as_float((uint32_t)lightNum));
-                                if (pend & PEND_LIGHT) st_spec(R->A, R->s_A, R->capacity, slot, dout.A, 0.f);
+                                st_beta_ld(R->direct[slot], R->s_beta_ld, slot, beta, pickPdf);
+                                R->direct[slot].sh_o = f4(dout.sh_o, __uint_as_float((uint32_t)lightNum));
+                                if (pend & PEND_LIGHT) st_spec(R->direct[slot].A, R->s_A, slot, dout.A, 0.f);
                                 if (pend & PEND_BSDF) {
-                                    R->mi_o[slot] = f4(dout.mi_o, 0.f);
-                                    R->mi_d[slot] = f4(dout.mi_d, 0.f);
-                                    st_spec(R->B, R->s_B, R->capacity, slot, dout.B, 0.f);
+                                    R->direct[slot].mi_o = f4(dout.mi_o, 0.f);
+                                    R->direct[slot].mi_d = f4(dout.mi_d, 0.f);
+                                    st_spec(R->direct[slot].B, R->s_B, slot, dout.B, 0.f);
                                 }
                             }
 #else
@@ -2342,17 +2358,18 @@ __global__ void __launch_bounds__(128, 4) k_medium(const RenderDev *R, int bounc
                                 float4 *sBl = reinterpret_cast<float4 *>(R->s_beta_ld + (size_t)slot * B200PT_NSPEC);
 #pragma unroll 5
                                 for (int q = 0; q < B200PT_NSPEC / 4; ++q) sBl[q] = sBeta[q];
-                                R->beta_ld[slot] = make_float4(0.f, 0.f, 0.f, pickPdf);
-                                R->sh_o[slot] = f4(dout.sh_o, __uint_as_float((uint32_t)lightNum));
-                                if (pend & PEND_LIGHT) R->A[slot] = make_float4(0.f, 0.f, 0.f, 0.f);
+                                R->direct[slot].beta_ld = make_float4(0.f, 0.f, 0.f, pickPdf);
+                                reset_direct_hits(R->direct[slot]);
+                                R->direct[slot].sh_o = f4(dout.sh_o, __uint_as_float((uint32_t)lightNum));
+                                if (pend & PEND_LIGHT) R->direct[slot].A = make_float4(0.f, 0.f, 0.f, 0.f);
                                 if (pend & PEND_BSDF) {
-                                    R->mi_o[slot] = f4(dout.mi_o, 0.f);
-                                    R->mi_d[slot] = f4(dout.mi_d, 0.f);
-                                    R->B[slot] = make_float4(0.f, 0.f, 0.f, 0.f);
+                                    R->direct[slot].mi_o = f4(dout.mi_o, 0.f);
+                                    R->direct[slot].mi_d = f4(dout.mi_d, 0.f);
+                                    R->direct[slot].B = make_float4(0.f, 0.f, 0.f, 0.f);
                                 }
                             }
 #endif
-                            R->sh_d[slot] = f4(dout.sh_d, __uint_as_float(pend));
+                            R->direct[slot].sh_d = f4(dout.sh_d, __uint_as_float(pend));
                         }
                     }
                     // mi.phase->Sample_p(wo, &wi, sampler.Get2D()); ray = mi.SpawnRay(wi) (volpath.cpp:95-98)
@@ -2398,12 +2415,12 @@ __global__ void __launch_bounds__(128, 4) k_medium(const RenderDev *R, int bounc
 #endif
                     if (cont) {
                         const uint32_t nmeta = ((uint32_t)st.dim & 0xffffu) | ((uint32_t)(bounces + 1) << 16);  // specularBounce = false
-                        R->ray_o[slot] = f4(no, etaScale);
-                        R->ray_d[slot] = f4(wi, __uint_as_float(nmeta));
+                        R->path[slot].o = f4(no, etaScale);
+                        R->path[slot].d = f4(wi, __uint_as_float(nmeta));
 #if B200PT_NSPEC == 3
-                        st_spec(R->beta, R->s_beta, R->capacity, slot, beta, 0.f);
+                        st_spec(R->path[slot].beta, R->s_beta, slot, beta, 0.f);
 #else
-                        R->beta[slot] = make_float4(0.f, 0.f, 0.f, 0.f);
+                        R->path[slot].beta = make_float4(0.f, 0.f, 0.f, 0.f);
 #endif
                     }
                 }
@@ -2472,20 +2489,20 @@ __global__ void __launch_bounds__(128, 4) k_medium_general(const RenderDev *R, i
         uint32_t pend = 0, slot = 0;
         if (active) {
             slot = queue[i];
-            const float4 o4 = R->ray_o[slot], d4 = R->ray_d[slot];
+            const float4 o4 = R->path[slot].o, d4 = R->path[slot].d;
             float betaW;
-            Spec beta = ld_spec(R->beta, R->s_beta, R->capacity, slot, &betaW);
+            Spec beta = ld_spec(R->path[slot].beta, R->s_beta, slot, &betaW);
             const V3 ro = v3(o4), rd = v3(d4);
             const float etaScale = o4.w;
             const uint32_t meta = __float_as_uint(d4.w);
             const int bounces = (int)((meta >> 16) & 0xffu);
             const int med = R->cur_med[slot];
-            const uint32_t ti = R->hit[slot];
+            const uint32_t ti = R->path[slot].hit;
             uint32_t mflags;
             const float tHit = hit_distance(R, ti, ro, rd, &mflags);
             const int bm = boundary_medium(R, ti);
             SobolStream st;
-            st.index = R->sobol[slot];
+            st.index = R->path[slot].sobol;
             st.dim = (int)(meta & 0xffffu);
             st.px = st.py = 0;
             const SamplerParams &sp = R->sampler;
@@ -2525,16 +2542,16 @@ __global__ void __launch_bounds__(128, 4) k_medium_general(const RenderDev *R, i
                             if (sphere_intersect(*bs, ro, rd, pt_inf(), &th, &is)) {
                                 R->cur_med[slot] = dot(rd, is.n) > 0 ? outside : bm;          // GetMedium(ray.d)
                                 const V3 no = offset_ray_origin(is.p, is.pError, is.n, rd);  // isect.SpawnRay(ray.d)
-                                R->ray_o[slot] = f4(no, etaScale);
-                                R->ray_d[slot] = f4(rd, __uint_as_float((meta & 0xffff0000u) | ((uint32_t)st.dim & 0xffffu)));
-                                st_spec(R->beta, R->s_beta, R->capacity, slot, beta, betaW);
+                                R->path[slot].o = f4(no, etaScale);
+                                R->path[slot].d = f4(rd, __uint_as_float((meta & 0xffff0000u) | ((uint32_t)st.dim & 0xffffu)));
+                                st_spec(R->path[slot].beta, R->s_beta, slot, beta, betaW);
                                 cross = true;
                             }
                         }
                     } else {
                         // on to the surface vertex (or out of the scene)
-                        st_spec(R->beta, R->s_beta, R->capacity, slot, beta, betaW);
-                        R->ray_d[slot] = f4(rd, __uint_as_float((meta & 0xffff0000u) | ((uint32_t)st.dim & 0xffffu)));
+                        st_spec(R->path[slot].beta, R->s_beta, slot, beta, betaW);
+                        R->path[slot].d = f4(rd, __uint_as_float((meta & 0xffff0000u) | ((uint32_t)st.dim & 0xffffu)));
                         if (ti != B200PT_MISS) family = R->scene.materials[mflags & 0xffffu].type;
                     }
                 } else if (bounces < R->max_depth) {  // volpath.cpp:84-85
@@ -2564,17 +2581,17 @@ __global__ void __launch_bounds__(128, 4) k_medium_general(const RenderDev *R, i
                             estimate_direct<true>(R, mi, none, uScattering, lightNum, uLight, &dout, true, med);
                             pend = dout.pend;
                             if (pend) {
-                                st_spec(R->beta_ld, R->s_beta_ld, R->capacity, slot, beta, pickPdf);
-                                R->sh_o[slot] = f4(dout.sh_o, __uint_as_float((uint32_t)lightNum));
-                                if (pend & PEND_LIGHT) st_spec(R->A, R->s_A, R->capacity, slot, dout.A, dout.wA);
+                                st_beta_ld(R->direct[slot], R->s_beta_ld, slot, beta, pickPdf);
+                                R->direct[slot].sh_o = f4(dout.sh_o, __uint_as_float((uint32_t)lightNum));
+                                if (pend & PEND_LIGHT) st_spec(R->direct[slot].A, R->s_A, slot, dout.A, dout.wA);
                                 if (pend & PEND_BSDF) {
-                                    R->mi_o[slot] = f4(dout.mi_o, dout.pdfB);
-                                    R->mi_d[slot] = f4(dout.mi_d, 0.f);
-                                    st_spec(R->B, R->s_B, R->capacity, slot, dout.B, dout.wB);
+                                    R->direct[slot].mi_o = f4(dout.mi_o, dout.pdfB);
+                                    R->direct[slot].mi_d = f4(dout.mi_d, 0.f);
+                                    st_spec(R->direct[slot].B, R->s_B, slot, dout.B, dout.wB);
                                 }
                                 store_direct_general(R, slot, dout, med);
                             }
-                            R->sh_d[slot] = f4(dout.sh_d, __uint_as_float(pend));
+                            R->direct[slot].sh_d = f4(dout.sh_d, __uint_as_float(pend));
                         }
                     }
                     V3 wi;
@@ -2593,9 +2610,9 @@ __global__ void __launch_bounds__(128, 4) k_medium_general(const RenderDev *R, i
                     }
                     if (cont) {
                         const uint32_t nmeta = ((uint32_t)st.dim & 0xffffu) | ((uint32_t)(bounces + 1) << 16);  // specularBounce = false
-                        R->ray_o[slot] = f4(no, etaScale);
-                        R->ray_d[slot] = f4(wi, __uint_as_float(nmeta));
-                        st_spec(R->beta, R->s_beta, R->capacity, slot, beta, 0.f);
+                        R->path[slot].o = f4(no, etaScale);
+                        R->path[slot].d = f4(wi, __uint_as_float(nmeta));
+                        st_spec(R->path[slot].beta, R->s_beta, slot, beta, 0.f);
                     }
                 }
             }
@@ -2636,14 +2653,14 @@ __global__ void __launch_bounds__(128, 4) k_direct_walk(const RenderDev *R, cons
         if (i < n) {
             slot = queue[i];
             if (SHADOW) {
-                const float4 o4 = R->sh_o[slot], d4 = R->sh_d[slot], tr4 = R->sh_tr[slot];
+                const float4 o4 = R->direct[slot].sh_o, d4 = R->direct[slot].sh_d, tr4 = R->sh_tr[slot];
                 const V3 o = v3(o4), d = v3(d4);
                 int m = (int)__float_as_uint(tr4.w);
                 Spec Tr = rgb(tr4.x, tr4.y, tr4.z);
                 const uint32_t ti = R->sh_hit[slot];
                 const int bm = boundary_medium(R, ti);
                 if (ti != B200PT_MISS && bm < 0) {
-                    R->occluded[slot] = 1;  // an opaque surface between the point and the light
+                    R->direct[slot].occluded = 1;  // an opaque surface between the point and the light
                 } else {
                     float th = PT_SHADOW_TMAX;
                     Isect ii;
@@ -2653,30 +2670,30 @@ __global__ void __launch_bounds__(128, 4) k_direct_walk(const RenderDev *R, cons
                     if (m >= 0) Tr = Tr * medium_tr(media_sigma_t(R, m), d, th);
                     if (!crossed) {
                         float wA;
-                        const Spec f = ld_spec(R->A, R->s_A, R->capacity, slot, &wA);
+                        const Spec f = ld_spec(R->direct[slot].A, R->s_A, slot, &wA);
                         const float4 l4 = R->A2[slot];
                         const Spec Li = rgb(l4.x, l4.y, l4.z) * Tr;
                         const Spec A = wA < 0.f ? f * Li / 1.f : f * Li * wA / l4.w;
-                        st_spec(R->A, R->s_A, R->capacity, slot, A, 0.f);
-                        R->occluded[slot] = 0;
+                        st_spec(R->direct[slot].A, R->s_A, slot, A, 0.f);
+                        R->direct[slot].occluded = 0;
                     } else {
                         const V3 p1 = v3(R->sh_p1[slot]), p1e = v3(R->sh_p1e[slot]), p1n = v3(R->sh_p1n[slot]);
                         const V3 o2 = offset_ray_origin(ii.p, ii.pError, ii.n, p1 - ii.p);
                         const V3 target = offset_ray_origin(p1, p1e, p1n, o2 - p1);
                         const V3 d2 = target - o2;
                         m = dot(d2, ii.n) > 0 ? outside : bm;  // GetMedium(d)
-                        R->sh_o[slot] = f4(o2, o4.w);
-                        R->sh_d[slot] = f4(d2, d4.w);
+                        R->direct[slot].sh_o = f4(o2, o4.w);
+                        R->direct[slot].sh_d = f4(d2, d4.w);
                         R->sh_tr[slot] = make_float4(Tr.c[0], Tr.c[1], Tr.c[2], __uint_as_float((uint32_t)m));
                         again = true;
                     }
                 }
             } else {
-                const float4 o4 = R->mi_o[slot], d4 = R->mi_d[slot], tr4 = R->mi_tr[slot];
+                const float4 o4 = R->direct[slot].mi_o, d4 = R->direct[slot].mi_d, tr4 = R->mi_tr[slot];
                 const V3 o = v3(o4), wi = v3(d4);
                 int m = (int)__float_as_uint(tr4.w);
                 Spec Tr = rgb(tr4.x, tr4.y, tr4.z);
-                const uint32_t ti = R->mis_hit[slot];
+                const uint32_t ti = R->direct[slot].mis_hit;
                 const int bm = boundary_medium(R, ti);
                 float th = pt_inf();
                 Isect ii;
@@ -2684,11 +2701,11 @@ __global__ void __launch_bounds__(128, 4) k_direct_walk(const RenderDev *R, cons
                     if (m >= 0) Tr = Tr * medium_tr(media_sigma_t(R, m), wi, th);
                     const V3 o2 = offset_ray_origin(ii.p, ii.pError, ii.n, wi);  // isect->SpawnRay(ray.d)
                     m = dot(wi, ii.n) > 0 ? outside : bm;
-                    R->mi_o[slot] = f4(o2, o4.w);
+                    R->direct[slot].mi_o = f4(o2, o4.w);
                     R->mi_tr[slot] = make_float4(Tr.c[0], Tr.c[1], Tr.c[2], __uint_as_float((uint32_t)m));
                     again = true;
                 } else {
-                    const int lightNum = (int)__float_as_uint(R->sh_o[slot].w);
+                    const int lightNum = (int)__float_as_uint(R->direct[slot].sh_o.w);
                     const DevLight light = R->lights[lightNum];
                     Spec B = rgb1(0.f);
                     if (ti != B200PT_MISS && ti == light.tri) {
@@ -2716,11 +2733,11 @@ __global__ void __launch_bounds__(128, 4) k_direct_walk(const RenderDev *R, cons
                         const Spec Le = (light.two_sided || dot(ln, -wi) > 0) ? light_emit(R, lightNum, light) : rgb1(0.f);
                         if (!is_black(Le)) {
                             float wB;
-                            const Spec f = ld_spec(R->B, R->s_B, R->capacity, slot, &wB);
+                            const Spec f = ld_spec(R->direct[slot].B, R->s_B, slot, &wB);
                             B = f * Le * Tr * wB / o4.w;
                         }
                     }
-                    st_spec(R->B, R->s_B, R->capacity, slot, B, 0.f);
+                    st_spec(R->direct[slot].B, R->s_B, slot, B, 0.f);
                 }
             }
         }
@@ -2738,45 +2755,47 @@ __global__ void __launch_bounds__(256) k_resolve(const RenderDev *R, int bounce,
     while (warp_fetch(work, n, &i)) {
         if (i >= n) continue;
         const uint32_t slot = queue[i];
-        const float4 sd = R->sh_d[slot];
+        DirectRec &D = R->direct[slot];
+        const float4 sd = D.sh_d;
         const uint32_t pend = __float_as_uint(sd.w);
         if (!pend) continue;
 #if B200PT_NSPEC == 3
         Spec Ld = rgb1(0.f);
         bool any = false;
-        if ((pend & PEND_LIGHT) && !R->occluded[slot]) {
+        if ((pend & PEND_LIGHT) && !D.occluded) {
             float w_;
-            Ld = Ld + ld_spec(R->A, R->s_A, R->capacity, slot, &w_);
+            Ld = Ld + ld_spec(D.A, R->s_A, slot, &w_);
             any = true;
         }
         if (pend & PEND_BSDF) {
-            const uint32_t lightNum = __float_as_uint(R->sh_o[slot].w);
+            const uint32_t lightNum = __float_as_uint(D.sh_o.w);
             float w_;
-            const Spec B = ld_spec(R->B, R->s_B, R->capacity, slot, &w_);
-            if (R->mis_hit[slot] == R->lights[lightNum].tri && !is_black(B)) {
+            const Spec B = ld_spec(D.B, R->s_B, slot, &w_);
+            if (D.mis_hit == R->lights[lightNum].tri && !is_black(B)) {
                 Ld = Ld + B;
                 any = true;
             }
         }
         if (any) {
             float pickPdf, LW;
-            const Spec betaLd = ld_spec(R->beta_ld, R->s_beta_ld, R->capacity, slot, &pickPdf);
-            const Spec L = ld_spec(R->L, R->s_L, R->capacity, slot, &LW) + betaLd * (Ld / pickPdf);
-            st_spec(R->L, R->s_L, R->capacity, slot, L, LW);
+            const Spec betaLd = ld_spec(D.beta_ld, R->s_beta_ld, slot, &pickPdf);
+            PathRec &P = R->path[slot];
+            const Spec L = ld_spec(P.L, R->s_L, slot, &LW) + betaLd * (Ld / pickPdf);
+            st_spec(P.L, R->s_L, slot, L, LW);
         }
 #else
         // 60 bins: streamed through the slot's rows, bin by bin (Ld = 0 + A + B; L += beta_ld * (Ld / pickPdf))
-        const bool takeA = (pend & PEND_LIGHT) && !R->occluded[slot];
+        const bool takeA = (pend & PEND_LIGHT) && !D.occluded;
         bool takeB = false;
         if (pend & PEND_BSDF) {
-            const uint32_t lightNum = __float_as_uint(R->sh_o[slot].w);
-            if (R->mis_hit[slot] == R->lights[lightNum].tri) {
+            const uint32_t lightNum = __float_as_uint(D.sh_o.w);
+            if (D.mis_hit == R->lights[lightNum].tri) {
                 const float *sB = R->s_B + (size_t)slot * B200PT_NSPEC;
                 for (int b = 0; b < B200PT_NSPEC && !takeB; ++b) takeB = sB[b] != 0.f;
             }
         }
         if (takeA || takeB) {
-            const float pickPdf = R->beta_ld[slot].w;
+            const float pickPdf = D.beta_ld.w;
             const float4 *sA = reinterpret_cast<const float4 *>(R->s_A + (size_t)slot * B200PT_NSPEC);
             const float4 *sB = reinterpret_cast<const float4 *>(R->s_B + (size_t)slot * B200PT_NSPEC);
             const float4 *sBl = reinterpret_cast<const float4 *>(R->s_beta_ld + (size_t)slot * B200PT_NSPEC);
@@ -2798,7 +2817,7 @@ __global__ void __launch_bounds__(256) k_resolve(const RenderDev *R, int bounce,
             }
         }
 #endif
-        R->sh_d[slot] = make_float4(sd.x, sd.y, sd.z, 0.f);
+        D.sh_d = make_float4(sd.x, sd.y, sd.z, 0.f);
     }
 }
 
@@ -2902,7 +2921,7 @@ __global__ void __launch_bounds__(256) k_sort_hist(const RenderDev *R, const uin
     const uint32_t n = *count;
     for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
         const uint32_t slot = queue[i];
-        const uint32_t key = coherence_key(R, ray_o[slot], ray_d[slot]);
+        const uint32_t key = coherence_key(R, ray_o[(size_t)slot * REC_F4], ray_d[(size_t)slot * REC_F4]);
         R->sort_keys[i] = key;
         atomicAdd(&R->sort_hist[key], 1u);
     }
@@ -2965,7 +2984,7 @@ __global__ void __launch_bounds__(18 * 18) k_film(const RenderDev *R, uint32_t f
             const uint32_t base = (tb * 256u + pix) * spp;
             for (uint32_t s = 0; s < spp; ++s) {
                 float vw;
-                Spec Lv = ld_spec(R->L, R->s_L, R->capacity, base + s, &vw);
+                Spec Lv = ld_spec(R->path[base + s].L, R->s_L, base + s, &vw);
                 if (!own) {
                     const uint32_t code = __float_as_uint(vw);
                     const bool cx = (X == sx) || (X == sx - 1 && (code & 1u)) || (X == sx + 1 && (code & 2u));
@@ -3047,7 +3066,7 @@ __global__ void __launch_bounds__(1024) k_film_tile(const RenderDev *R, uint32_t
                     const int ifx = min((int)floorf(fx), 15), ify = min((int)floorf(fy), 15);
                     const float w = R->filter_table[ify * 16 + ifx];
                     float vw;
-                    Spec Lv = ld_spec(R->L, R->s_L, R->capacity, (uint32_t)(base + s), &vw);
+                    Spec Lv = ld_spec(R->path[(uint32_t)(base + s)].L, R->s_L, (uint32_t)(base + s), &vw);
                     // integrator.cpp:294-315
                     if (has_nans(Lv))
                         Lv = rgb1(0.f);

@@ -6,8 +6,8 @@
 // i.e. the reference's loop nest tile -> pixel (row-major) -> sample flattened,
 // so a warp holds 32 consecutive samples of one pixel (coherent camera rays)
 // and the film kernel can re-create the reference's per-tile summation order.
-// Per-slot state lives in float4-packed SoA arrays (one coalesced 16-byte
-// access per thread); queues of slot indices connect the stages.
+// Per-slot state lives in two 128-byte records per slot (PathRec, DirectRec);
+// queues of slot indices connect the stages.
 #ifndef B200PT_KERNELS_CUH
 #define B200PT_KERNELS_CUH
 
@@ -58,6 +58,38 @@ enum { PF_SPECULAR = 1 };
 // pending direct-lighting flags
 enum { PEND_LIGHT = 1, PEND_BSDF = 2 };
 
+// Per-slot state.  Every kernel after raygen reaches its slots through a queue, so the slots a warp touches are scattered
+// and each access costs whole 32-byte sectors.  The state is therefore kept in two records of four sectors per slot:
+// a sector holds fields of one slot only, the fields one kernel uses together share a sector, and a kernel that rewrites
+// a sector writes all of it where it has the values.  Both records are 128 bytes, so one stride indexes either.
+// SampledSpectrum build: the float4 spectra (beta, L, A, B, beta_ld) keep only their fourth component; the 60 bins live in
+// the slot-major RenderDev::s_* arrays.
+struct alignas(128) PathRec {
+    float4 o;            // [0] ray origin, etaScale             the traversal fetches the ray as this one sector
+    float4 d;            //     ray direction, meta (bits)
+    float4 beta;         // [1] beta.rgb, 0
+    float4 L;            //     L.rgb, bleed code (bits)
+    uint64_t sobol;      // [2] Sobol' index of (pixel, sample)
+    uint32_t hit;        //     closest-hit triangle (leaf order) of the path ray
+    uint32_t hit_inst;   //     instance of that hit when the triangle belongs to an object (scenes with instances)
+    uint32_t unused[12];
+};
+struct alignas(128) DirectRec {
+    float4 sh_o;         // [0] shadow ray origin, light number (bits)     the any-hit traversal's ray
+    float4 sh_d;         //     shadow ray direction, pending flags (bits)
+    float4 mi_o;         // [1] MIS (BSDF-sampled) ray origin, scattering pdf   the MIS traversal's ray
+    float4 mi_d;         //     MIS ray direction
+    float4 A;            // [2] light-sampling term f*Li*w/lightPdf
+    float4 B;            //     BSDF-sampling term f*Le*w/scatteringPdf, valid if the MIS ray reaches the light
+    float4 beta_ld;      // [3] beta at the time of the direct-lighting estimate, light pick pdf
+    uint32_t mis_hit;    //     closest-hit triangle of the MIS ray
+    uint8_t occluded;    //     any-hit result of the shadow ray
+    uint8_t unused[11];
+};
+static_assert(sizeof(PathRec) == 128 && sizeof(DirectRec) == 128, "per-slot records are four 32-byte sectors");
+// float4 stride of the ray pairs (PathRec::o/d, DirectRec::sh_o/sh_d, DirectRec::mi_o/mi_d) from one slot to the next
+constexpr int REC_F4 = (int)(sizeof(PathRec) / sizeof(float4));
+
 struct RenderDev {
     DevScene scene;
     SamplerParams sampler;
@@ -92,25 +124,11 @@ struct RenderDev {
     int tiles_x, tiles_y;
     const int32_t *tile_list;  // tile ids of the whole render_tiles call
     uint32_t capacity;         // path slots per batch
-    // per-slot state (float4-packed)
-    float4 *ray_o;     // o.xyz, etaScale
-    float4 *ray_d;     // d.xyz, meta (bits)
-    float4 *beta;      // beta.rgb, light pick pdf
-    float4 *L;         // L.rgb, bleed code (bits)
-    uint64_t *sobol;   // Sobol' index of (pixel, sample)
-    uint32_t *hit;     // closest-hit triangle (leaf order) of the path ray
-    uint32_t *hit_inst; // instance of that hit when the triangle belongs to an object (scenes with instances)
-    float4 *sh_o;      // shadow ray origin, light number (bits)
-    float4 *sh_d;      // shadow ray direction, pending flags (bits)
-    float4 *A;         // light-sampling term  f*Li*w/lightPdf
-    float4 *mi_o;      // MIS (BSDF-sampled) ray origin
-    float4 *mi_d;      // MIS ray direction
-    float4 *B;         // BSDF-sampling term f*Le*w/scatteringPdf, valid if the MIS ray reaches the light
-    float4 *beta_ld;   // beta at the time of the direct-lighting estimate
-    uint8_t *occluded; // any-hit result of the shadow ray
-    uint32_t *mis_hit; // closest-hit triangle of the MIS ray
+    // per-slot state
+    PathRec *path;
+    DirectRec *direct;
     // SampledSpectrum build only (nullptr otherwise): the bins of beta, L, A, B and beta_ld, slot-major [capacity][60]
-    // (240 contiguous bytes per slot, see ld_spec); the float4 arrays above then keep just their fourth component
+    // (240 contiguous bytes per slot, see ld_spec); the float4 fields of the records then keep just their fourth component
     float *s_beta, *s_L, *s_A, *s_B, *s_beta_ld;
     const float *light_spectra;  // [n_lights][60]: Lemit / I / L of each light
     uint8_t *pix_bleed;  // [tiles_per_batch*256] pixel has a sample whose box-filter footprint leaves the pixel
@@ -169,10 +187,11 @@ struct TraceArgs {
     uint32_t *work;        // persistent fetch counter (zeroed)
     float fixed_t_max;     // used unless t_max_from_w
     int t_max_from_w;
-    int stride;            // ray_o/ray_d element stride in float4 (1 for SoA state, 2 for b200pt_ray)
+    int stride;            // ray_o/ray_d element stride in float4 (REC_F4 for the per-slot records, 2 for b200pt_ray)
     uint32_t *hit_out;     // closest: triangle per slot
     b200pt_hit *full_out;  // closest: optional full record (prim id, t, b0, b1)
     uint8_t *occ_out;      // any-hit result per slot
+    int out_stride;        // bytes from one slot's hit_out / hit_inst_out / occ_out entry to the next (see slot_out)
     // classification of closest hits by material family
     uint32_t *q_mat[4];
     uint32_t *qcount_mat;  // &qcount[bounce*Q_PER_BOUNCE + Q_MAT0]
@@ -195,6 +214,11 @@ struct TraceArgs {
     uint32_t tlas_node_off, tlas_tri_off;  // see DevScene
     uint32_t *hit_inst_out;     // instance of an object-triangle hit (closest, render path)
 };
+// the entry of `slot` in a traversal output: a field of the per-slot records or an element of a plain array
+template <class T>
+__device__ __forceinline__ T &slot_out(T *base, uint32_t slot, int stride) {
+    return *reinterpret_cast<T *>(reinterpret_cast<char *>(base) + (size_t)slot * (size_t)stride);
+}
 
 void launch_raygen(const RenderDev *dev, uint32_t batch_first_tile, uint32_t n_batch_tiles, uint32_t n_slots,
                    cudaStream_t s);
@@ -224,6 +248,7 @@ void launch_direct_walk(const RenderDev *dev, const RenderDev &host, bool shadow
 #define SORT_BUCKETS (1u << 18)  // 3 octant bits + 15 Morton bits
 // Counting sort of a queue of slots by the coherence key of the rays they refer to; `out` receives
 // the permuted queue (order inside a bucket is arbitrary -- it never affects a path's arithmetic).
+// ray_o / ray_d point at the ray pair of slot 0 in the per-slot records (stride REC_F4).
 void launch_sort_queue(const RenderDev *dev, const RenderDev &host, const uint32_t *queue, const uint32_t *count,
                        const float4 *ray_o, const float4 *ray_d, int grid, cudaStream_t s);
 void launch_sobol_table(const uint32_t *mat32, uint32_t *table, int n_dims, cudaStream_t s);
