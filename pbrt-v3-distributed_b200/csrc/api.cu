@@ -1127,8 +1127,9 @@ int b200pt_render_create(b200pt_scene *scene, const b200pt_camera_desc *cam, con
 
     // batch sizing: whole tiles, about B200PT_BATCH_PATHS path slots
     // path slots per batch: 256 B of records + ~40 B of queues each, plus 5 x 60 floats with a SampledSpectrum host.
-    // Larger batches keep the traversal launches fuller: RGB takes 32 Mi slots (~10 GB); 60 bins keep 16 Mi (~25 GB).
-    size_t target = scene->nspec ? (16u << 20) : (32u << 20);
+    // Larger batches keep the traversal launches fuller and spread each launch's drain over more rays: RGB takes 96 Mi slots
+    // (~29 GB; cfg4 on an H100 at 400 W: +3.5 % over 32 Mi, +0.9 % over 64 Mi, profiles/README.md); 60 bins keep 16 Mi (~25 GB).
+    size_t target = scene->nspec ? (16u << 20) : (96u << 20);
     if (const char *e = getenv("B200PT_BATCH_PATHS")) target = (size_t)atoll(e);
     const size_t per_tile = 256u * (size_t)r->spp;
     r->tiles_per_batch = (uint32_t)std::max<size_t>(1, target / per_tile);
