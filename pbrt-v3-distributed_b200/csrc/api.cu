@@ -66,7 +66,6 @@ struct b200pt_scene {
     b200pt_material *d_materials = nullptr;
     F4 *d_tri_n = nullptr, *d_tri_uv = nullptr;
     uint64_t n_nodes = 0, n_tris = 0;
-    uint64_t n_top_nodes = 0;  // nodes of the top-level tree (the first ones of d_nodes)
     std::vector<b200pt_material> materials;
     std::vector<b200pt_area_light> lights;  // host copy, triangle = original index
     std::vector<uint32_t> prim_to_tri;
@@ -105,9 +104,8 @@ struct b200pt_render {
     uint32_t *d_walk_counts = nullptr;  // bounded media: [16] queue counters / fetch counters of the boundary passes
     int grid_trace = 0, grid_shade = 0, grid_shade_s60 = 0;
     bool instrumented = false, profiling = false;
-    int refill_lanes = 26, postpone_pct = 40, trace_ctas = 0, stage_nodes = 0;  // k_trace knobs (b200pt_render_set_option)
+    int refill_lanes = 26, postpone_pct = 40;  // k_trace knobs (b200pt_render_set_option)
     bool overlap = true;  // run shadow/MIS rays of bounce b concurrently with the path rays of bounce b+1
-    int sort_from_bounce = -1;  // coherence-sort the path / shadow queues from this bounce on (<0: never; measured: no gain on the soups)
     std::vector<TimedLaunch> timed;
     std::vector<cudaEvent_t> event_pool;
     double ms[3] = {0, 0, 0};
@@ -157,7 +155,19 @@ static void trace_args_scene(TraceArgs &a, const b200pt_scene *s) {
     a.bounds = s->trav_bounds;
     a.tlas_bounds = s->tlas_bounds;
     a.tris = s->d_tris;
-    a.magic = 0x47000000u;
+}
+// the members every traversal launch of a render shares: the tree's, plus the per-slot record stride and the k_trace knobs;
+// everything else zero
+static TraceArgs trace_args_render(const b200pt_render *r) {
+    TraceArgs a;
+    memset(&a, 0, sizeof(a));
+    trace_args_scene(a, r->scene);
+    a.materials = r->host.scene.materials;
+    a.stats = r->host.stats;
+    a.stride = REC_F4;
+    a.refill_lanes = r->refill_lanes;
+    a.postpone_pct = r->postpone_pct;
+    return a;
 }
 
 extern "C" {
@@ -292,7 +302,6 @@ int b200pt_scene_create(b200pt_ctx *ctx, const b200pt_scene_desc *d, b200pt_scen
     std::vector<TravBounds> obj_bounds(obj_ranges.size());
     Wbvh bvh;
     GpuBuildOutput gout;
-    uint64_t n_top_nodes = 0;
     if (gpu_build) {
         // ---- on-device build (wbvh_gpu.cu): Morton order -> binary radix tree -> 7-wide collapse
         GpuBuildInput gin;
@@ -349,7 +358,6 @@ int b200pt_scene_create(b200pt_ctx *ctx, const b200pt_scene_desc *d, b200pt_scen
         int64_t bad = validate_wbvh(bvh);
         if (bad) return b200pt_fail(B200PT_ERR_INVALID, "scene_create: BVH validation found %lld violations", (long long)bad);
     }
-    n_top_nodes = bvh.nodes.size();
     // one tree per object, appended behind the top-level one; k_spheres traverses them through offset pointers,
     // so their node / triangle indices stay relative to the object's own arrays
     bvh.prim_to_tri.resize((size_t)d->n_triangles, 0xffffffffu);
@@ -480,7 +488,6 @@ int b200pt_scene_create(b200pt_ctx *ctx, const b200pt_scene_desc *d, b200pt_scen
     b200pt_scene *s = new b200pt_scene;
     s->ctx = ctx;
     s->n_nodes = n_node_records;
-    s->n_top_nodes = gpu_build ? (uint64_t)gout.n_nodes : n_top_nodes;
     s->n_tris = n_tri_records;
     s->materials.assign(d->materials, d->materials + d->n_materials);
     s->lights.assign(d->lights, d->lights + d->n_lights);
@@ -704,7 +711,7 @@ int b200pt_scene_info(const b200pt_scene *s, uint64_t *node_bytes, uint64_t *tri
 }
 
 // ------------------------------------------------- ray-batch entry points
-static int trace_grid(const b200pt_ctx *ctx) { return ctx->sm_count; }  // launch_trace multiplies by its CTAs per SM
+static int trace_grid(const b200pt_ctx *ctx) { return ctx->sm_count; }  // launch_trace multiplies by B200PT_TRACE_CTAS
 static int postpone_pct() {
     static int v = getenv("B200PT_POSTPONE_PCT") ? atoi(getenv("B200PT_POSTPONE_PCT")) : 40;
     return v;
@@ -715,14 +722,6 @@ static int refill_lanes() {
 }
 static int sphere_refill_lanes() {
     static int v = getenv("B200PT_SPHERE_REFILL") ? atoi(getenv("B200PT_SPHERE_REFILL")) : 8;
-    return v;
-}
-static int trace_ctas_default() {
-    static int v = getenv("B200PT_TRACE_CTAS_RT") ? atoi(getenv("B200PT_TRACE_CTAS_RT")) : 0;
-    return v;
-}
-static int stage_nodes_default() {
-    static int v = getenv("B200PT_STAGE_NODES") ? atoi(getenv("B200PT_STAGE_NODES")) : 0;
     return v;
 }
 
@@ -760,8 +759,6 @@ static int trace_dev(b200pt_scene *s, uint64_t rays_dev, uint64_t out_dev, int64
     a.materials = s->d_materials;
     a.refill_lanes = refill_lanes();
     a.postpone_pct = postpone_pct();
-    a.ctas = trace_ctas_default();
-    a.n_staged = (uint32_t)std::min<uint64_t>((uint64_t)std::max(0, stage_nodes_default()), s->n_top_nodes);
     if (any_hit)
         a.occ_out = reinterpret_cast<uint8_t *>(out_dev);
     else
@@ -1119,14 +1116,8 @@ int b200pt_render_create(b200pt_scene *scene, const b200pt_camera_desc *cam, con
                                nvox, nl);
         }
     }
-    for (int a = 0; a < 3; ++a) {
-        const float ext = scene->bounds_hi[a] - scene->bounds_lo[a];
-        H.sort_lo[a] = scene->bounds_lo[a];
-        H.sort_inv[a] = ext > 0 ? 32.f / ext : 0.f;
-    }
-
     // batch sizing: whole tiles, about B200PT_BATCH_PATHS path slots
-    // path slots per batch: 256 B of records + ~40 B of queues each, plus 5 x 60 floats with a SampledSpectrum host.
+    // path slots per batch: 256 B of records + 32 B of queues each, plus 5 x 60 floats with a SampledSpectrum host.
     // Larger batches keep the traversal launches fuller and spread each launch's drain over more rays: RGB takes 96 Mi slots
     // (~29 GB; cfg4 on an H100 at 400 W: +3.5 % over 32 Mi, +0.9 % over 64 Mi, profiles/README.md); 60 bins keep 16 Mi (~25 GB).
     size_t target = scene->nspec ? (16u << 20) : (96u << 20);
@@ -1198,9 +1189,6 @@ int b200pt_render_create(b200pt_scene *scene, const b200pt_camera_desc *cam, con
     ALLOC(H.q_path[1], cap);
     for (int m = 0; m < 4; ++m) ALLOC(H.q_mat[m], cap);
     ALLOC(H.q_shadow, cap);
-    ALLOC(H.q_sorted, cap);
-    ALLOC(H.sort_keys, cap);
-    ALLOC(H.sort_hist, (size_t)SORT_BUCKETS);
     ALLOC(H.q_mis, cap);
     ALLOC(H.qcount, (size_t)(H.max_depth + 2) * Q_PER_BOUNCE);
     ALLOC(H.work, (size_t)(H.max_depth + 2) * 16);
@@ -1313,19 +1301,16 @@ int b200pt_render_create(b200pt_scene *scene, const b200pt_camera_desc *cam, con
         CUDA_TRY(cudaGetLastError());
     }
     CUDA_TRY(cudaStreamSynchronize(st));
-    r->grid_trace = ctx->sm_count;  // launch_trace multiplies by its CTAs per SM
+    r->grid_trace = ctx->sm_count;  // launch_trace multiplies by B200PT_TRACE_CTAS
     r->grid_shade = ctx->sm_count * 8;
     // grid of the 60-bin shading kernels in CTAs per SM (B200PT_S60_SHADE_CTAS; a knob from the time they kept their
     // spectra in multi-KB local-memory frames -- with lazy spectra the frame is about 1 KB)
     r->grid_shade_s60 = ctx->sm_count * (getenv("B200PT_S60_SHADE_CTAS") ? std::max(1, atoi(getenv("B200PT_S60_SHADE_CTAS"))) : 8);
     if (getenv("B200PT_INSTRUMENT")) r->instrumented = atoi(getenv("B200PT_INSTRUMENT")) != 0;
     if (getenv("B200PT_PROFILE")) r->profiling = atoi(getenv("B200PT_PROFILE")) != 0;
-    if (getenv("B200PT_SORT_FROM")) r->sort_from_bounce = atoi(getenv("B200PT_SORT_FROM"));
     if (getenv("B200PT_OVERLAP")) r->overlap = atoi(getenv("B200PT_OVERLAP")) != 0;
     r->refill_lanes = refill_lanes();
     r->postpone_pct = postpone_pct();
-    r->trace_ctas = trace_ctas_default();
-    r->stage_nodes = stage_nodes_default();
     render_guard.p = nullptr;
     *out = r;
     return B200PT_OK;
@@ -1465,7 +1450,7 @@ int b200pt_render_tiles(b200pt_render *r, const int32_t *tiles, int64_t n_tiles)
             if (cudaStreamSynchronize(s_) != cudaSuccess) return 0u;
             return v;
         };
-        const bool overlap = r->overlap && r->sort_from_bounce < 0 && !medium;
+        const bool overlap = r->overlap && !medium;
         cudaStream_t st2 = overlap ? ctx->stream_aux : st;
         const bool tl = two_level(r->scene) && !r->instrumented;  // instances inside the traversal kernel
         const bool has_spheres = H.scene.n_spheres > 0 || (H.scene.n_instances > 0 && !tl);  // "extra shapes" pass needed
@@ -1501,26 +1486,12 @@ int b200pt_render_tiles(b200pt_render *r, const int32_t *tiles, int64_t n_tiles)
         auto trace_path = [&](int b) {
             uint32_t *qc = H.qcount + (size_t)b * Q_PER_BOUNCE;
             uint32_t *wk = H.work + (size_t)b * 16;
-            TraceArgs a;
-            memset(&a, 0, sizeof(a));
-            trace_args_scene(a, r->scene);
-            a.materials = H.scene.materials;
-            a.stats = H.stats;
-            a.stride = REC_F4;
+            TraceArgs a = trace_args_render(r);
             a.out_stride = (int)sizeof(PathRec);
-            a.refill_lanes = r->refill_lanes;
-            a.postpone_pct = r->postpone_pct;
-            a.ctas = r->trace_ctas;
-            a.n_staged = (uint32_t)std::min<uint64_t>((uint64_t)std::max(0, r->stage_nodes), r->scene->n_top_nodes);
             // closest hit of the path rays + classification by BSDF family
-            const bool sorted = r->sort_from_bounce >= 0 && b >= r->sort_from_bounce;
-            if (sorted) {
-                LaunchTimer lt(r, st, 2);
-                launch_sort_queue(r->d_dev, H, H.q_path[b & 1], qc + Q_PATH, &H.path->o, &H.path->d, r->grid_shade, st);
-            }
             a.ray_o = &H.path->o;
             a.ray_d = &H.path->d;
-            a.queue = sorted ? H.q_sorted : H.q_path[b & 1];
+            a.queue = H.q_path[b & 1];
             a.count = qc + Q_PATH;
             a.work = wk + 0;
             a.fixed_t_max = INFINITY;
@@ -1577,15 +1548,7 @@ int b200pt_render_tiles(b200pt_render *r, const int32_t *tiles, int64_t n_tiles)
         auto walk_direct = [&](int b, bool shadow) {
             uint32_t *qc = H.qcount + (size_t)b * Q_PER_BOUNCE;
             uint32_t *wk = H.work + (size_t)b * 16;
-            TraceArgs a;
-            memset(&a, 0, sizeof(a));
-            trace_args_scene(a, r->scene);
-            a.materials = H.scene.materials;
-            a.stats = H.stats;
-            a.stride = REC_F4;
-            a.refill_lanes = r->refill_lanes;
-            a.postpone_pct = r->postpone_pct;
-            a.ctas = r->trace_ctas;
+            TraceArgs a = trace_args_render(r);
             a.ray_o = shadow ? &H.direct->sh_o : &H.direct->mi_o;
             a.ray_d = shadow ? &H.direct->sh_d : &H.direct->mi_d;
             a.fixed_t_max = shadow ? PT_SHADOW_TMAX : INFINITY;
@@ -1631,26 +1594,12 @@ int b200pt_render_tiles(b200pt_render *r, const int32_t *tiles, int64_t n_tiles)
             }
             uint32_t *qc = H.qcount + (size_t)b * Q_PER_BOUNCE;
             uint32_t *wk = H.work + (size_t)b * 16;
-            TraceArgs a;
-            memset(&a, 0, sizeof(a));
-            trace_args_scene(a, r->scene);
-            a.materials = H.scene.materials;
-            a.stats = H.stats;
-            a.stride = REC_F4;
+            TraceArgs a = trace_args_render(r);
             a.out_stride = (int)sizeof(DirectRec);
-            a.refill_lanes = r->refill_lanes;
-            a.postpone_pct = r->postpone_pct;
-            a.ctas = r->trace_ctas;
-            a.n_staged = (uint32_t)std::min<uint64_t>((uint64_t)std::max(0, r->stage_nodes), r->scene->n_top_nodes);
             // shadow rays (any hit), tMax = 1 - ShadowEpsilon
-            const bool sorted_sh = r->sort_from_bounce >= 0;
-            if (sorted_sh) {
-                LaunchTimer lt(r, st2, 2);
-                launch_sort_queue(r->d_dev, H, H.q_shadow, qc + Q_SHADOW, &H.direct->sh_o, &H.direct->sh_d, r->grid_shade, st2);
-            }
             a.ray_o = &H.direct->sh_o;
             a.ray_d = &H.direct->sh_d;
-            a.queue = sorted_sh ? H.q_sorted : H.q_shadow;
+            a.queue = H.q_shadow;
             a.count = qc + Q_SHADOW;
             a.work = wk + 5;
             a.fixed_t_max = PT_SHADOW_TMAX;
@@ -2032,10 +1981,6 @@ int b200pt_render_set_option(b200pt_render *r, const char *name, int value) {
         r->refill_lanes = value;
     else if (!strcmp(name, "postpone_pct"))
         r->postpone_pct = value;
-    else if (!strcmp(name, "trace_ctas"))
-        r->trace_ctas = value;
-    else if (!strcmp(name, "stage_nodes"))
-        r->stage_nodes = value < 0 ? 0 : (value > 512 ? 512 : value);
     else if (!strcmp(name, "overlap"))
         r->overlap = value != 0;
     else

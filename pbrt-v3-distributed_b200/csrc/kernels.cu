@@ -350,94 +350,12 @@ __device__ __forceinline__ void ray_store_hit(float *col, const TravRay &R) {
     col[12 * 128] = R.hit.b2;
 }
 
-__device__ __forceinline__ uint32_t smem_u32(const void *p) { return (uint32_t)__cvta_generic_to_shared(p); }
-
-// CTAS: resident CTAs per SM the kernel is compiled for (register budget); STAGE: the top of the tree is staged in
-// shared memory by TMA (cp.async.bulk + mbarrier; an experiment variant, off in the product build).
-// Experiment (off): with B200PT_SMEM_STACK = n the first n entries of a lane's traversal stack live in shared memory, one
-// column per thread (lanes at different depths hit different rows but their own bank: a push or pop of the whole warp is
-// two conflict-free wavefronts instead of one L1 tag lookup per distinct depth in local memory); deeper entries go to local
-// memory.  It showed no gain for 8 KB of shared memory per CTA, so the stack stays in local memory.
-#ifndef B200PT_SMEM_STACK
-#define B200PT_SMEM_STACK 0
-#endif
-// Parked triangle groups per lane (see the traversal loop of k_trace): 1 = one group in registers; 2 = a second one in
-// shared memory, so that the triangle phase starts with more lanes on board.
-#ifndef B200PT_PARK_DEPTH
-#define B200PT_PARK_DEPTH 1
-#endif
-// Triangle phase as a warp-wide work list (1) or per lane (0).  Per lane, a lane with three triangles loops three times
-// while lanes without any wait, so few lanes are active over the phase's instructions.  With the list, the lanes that
-// parked a group publish (lane, triangle)
-// pairs in shared memory and every converged lane takes one pair: the ray is read from its owner's column of s_ray, the
-// closest candidate per owner is settled with a 64-bit shared-memory atomicMin on (t, position in the list), the winner
-// writes the hit into the owner's column.
-#ifndef B200PT_TRI_SHARE
-#define B200PT_TRI_SHARE 0
-#endif
-#define B200PT_PAIR_CAP 64
-struct LaneStack {
-    uint32_t *sx, *sy;  // this thread's column of the shared part: entry e at [e * 128]
-    uint32_t x[B200PT_STACK - B200PT_SMEM_STACK], y[B200PT_STACK - B200PT_SMEM_STACK];
-    __device__ __forceinline__ void push(int sp, uint32_t gx, uint32_t gy) {
-        if (sp < B200PT_SMEM_STACK) {
-            sx[sp * 128] = gx;
-            sy[sp * 128] = gy;
-        } else {
-            x[sp - B200PT_SMEM_STACK] = gx;
-            y[sp - B200PT_SMEM_STACK] = gy;
-        }
-    }
-    __device__ __forceinline__ void pop(int sp, uint32_t *gx, uint32_t *gy) const {
-        if (sp < B200PT_SMEM_STACK) {
-            *gx = sx[sp * 128];
-            *gy = sy[sp * 128];
-        } else {
-            *gx = x[sp - B200PT_SMEM_STACK];
-            *gy = y[sp - B200PT_SMEM_STACK];
-        }
-    }
-};
-
-template <bool ANY_HIT, bool CLASSIFY, bool COUNT, int CTAS, bool STAGE>
-__global__ void __launch_bounds__(128, CTAS) k_trace(const TraceArgs a) {
+template <bool ANY_HIT, bool CLASSIFY, bool COUNT>
+__global__ void __launch_bounds__(128, B200PT_TRACE_CTAS) k_trace(const TraceArgs a) {
     // the slot-permutation table of the node test (wbvh_traverse.cuh), one copy per CTA
     __shared__ __align__(16) uint8_t s_lut[B200PT_LUT_BYTES];
     __shared__ float s_ray[B200PT_RAY_WORDS * 128];
-#if B200PT_SMEM_STACK > 0
-    __shared__ uint32_t s_stack[2 * B200PT_SMEM_STACK * 128];
-#endif
-#if B200PT_PARK_DEPTH > 1
-    __shared__ uint32_t s_park[2 * 128];  // a lane's second parked triangle group (x, y)
-#endif
-#if B200PT_TRI_SHARE
-    __shared__ uint32_t s_pairs[4 * B200PT_PAIR_CAP];  // per warp: owner lane << 27 | triangle
-    __shared__ unsigned long long s_key[128];          // per owner: min over its pairs of (t bits << 32 | list position)
-    __shared__ uint32_t s_cnt[4];
-#endif
-    __shared__ __align__(8) unsigned long long s_bar;
-    extern __shared__ __align__(128) uint8_t s_top[];  // STAGE: WbvhNode[a.n_staged]
     reinterpret_cast<uint4 *>(s_lut)[threadIdx.x] = __ldg(reinterpret_cast<const uint4 *>(a.lut) + threadIdx.x);
-    if (STAGE) {
-        if (threadIdx.x == 0) {
-            asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" ::"r"(smem_u32(&s_bar)));
-            asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-        }
-        __syncthreads();
-        if (threadIdx.x == 0) {
-            const uint32_t bytes = a.n_staged * 64u;
-            asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(&s_bar)), "r"(bytes) : "memory");
-            asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" ::"r"(smem_u32(s_top)),
-                         "l"(a.nodes), "r"(bytes), "r"(smem_u32(&s_bar))
-                         : "memory");
-        }
-        uint32_t done = 0;
-        while (!done)
-            asm volatile("{\n.reg .pred p;\nmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\nselp.u32 %0, 1, 0, p;\n}"
-                         : "=r"(done)
-                         : "r"(smem_u32(&s_bar)), "r"(0u)
-                         : "memory");
-    }
     __syncthreads();
     float *const my_ray = s_ray + threadIdx.x;
     const uint32_t n = *a.count;
@@ -445,18 +363,8 @@ __global__ void __launch_bounds__(128, CTAS) k_trace(const TraceArgs a) {
     TraceCounters ctr;
     ctr.nodes = ctr.tris = 0;
     Trav T;
-#if B200PT_SMEM_STACK > 0
-    LaneStack S;
-    S.sx = s_stack + threadIdx.x;
-    S.sy = s_stack + B200PT_SMEM_STACK * 128 + threadIdx.x;
-#else
     TravStack S;
-#endif
     uint32_t slot = 0, pend_x = 0, pend_y = 0;
-#if B200PT_PARK_DEPTH > 1
-    uint32_t *const my_park = s_park + threadIdx.x;
-    my_park[128] = 0;
-#endif
     bool has = false, fin = false, exhausted = false;
     while (true) {
         // ---- converged: retire finished rays
@@ -530,20 +438,11 @@ __global__ void __launch_bounds__(128, CTAS) k_trace(const TraceArgs a) {
             uint32_t ng_x = 0, ng_y = 0;
             const bool node_work = (T.cur_y & 0xff000000u) != 0;
             if (node_work)
-                trav_node_phase<!ANY_HIT, COUNT, STAGE>(T, S, a.nodes, a.tri_base, s_lut, &ng_x, &ng_y, &ctr,
-                                                        reinterpret_cast<const U4 *>(s_top), a.n_staged);
+                trav_node_phase<!ANY_HIT, COUNT>(T, S, a.nodes, a.tri_base, s_lut, &ng_x, &ng_y, &ctr);
             bool must = false;
             if (ng_y) {
                 if (pend_y) {
-#if B200PT_PARK_DEPTH > 1
-                    // a second group waits in shared memory; only a third one forces the triangle phase
-                    if (my_park[128] == 0) {
-                        my_park[0] = ng_x;
-                        my_park[128] = ng_y;
-                        ng_y = 0;
-                    } else
-#endif
-                        must = true;  // no room: flush the oldest parked group now, park the new one after
+                    must = true;  // no room: flush the parked group now, park the new one after
                 } else {
                     pend_x = ng_x;
                     pend_y = ng_y;
@@ -562,94 +461,6 @@ __global__ void __launch_bounds__(128, CTAS) k_trace(const TraceArgs a) {
             // only waiting for it that the node phase itself would run half empty
             if ((counts & 0xff00u) || n_parked * 100 >= n_act * a.postpone_pct || n_starving * 4 >= n_act) {
                 bool done = false;
-#if B200PT_TRI_SHARE
-                {
-                    const int warp = threadIdx.x >> 5;
-                    uint32_t *const wp = s_pairs + warp * B200PT_PAIR_CAP;
-                    float *const warp_rays = s_ray + (threadIdx.x & ~31);
-                    uint32_t tg_x = 0, tg_y = 0;
-                    if (pend_y) leaf_group_triangles(a.tri_base, pend_x, pend_y, &tg_x, &tg_y);
-                    const uint32_t cnt = (uint32_t)__popc(tg_y);
-                    if (COUNT) ctr.tris += cnt;
-                    if (lane == __ffs(act) - 1) s_cnt[warp] = 0;
-                    __syncwarp(act);
-                    uint32_t pos = 0;
-                    if (cnt) {
-                        pos = atomicAdd(&s_cnt[warp], cnt);
-                        s_key[threadIdx.x] = ~0ull;
-                    }
-                    // a group that does not fit the list (or a triangle index too large for the pair word) stays with its lane
-                    const bool own = cnt && (pos + cnt > B200PT_PAIR_CAP || tg_x + 32u >= (1u << 27));
-                    if (cnt) {
-                        uint32_t bits = tg_y, k = pos;
-                        while (bits && k < B200PT_PAIR_CAP) {
-                            const int j = msb32(bits);
-                            bits &= ~(1u << j);
-                            wp[k++] = own ? 0xffffffffu : (((uint32_t)lane << 27) | (tg_x + (uint32_t)j));
-                        }
-                    }
-                    __syncwarp(act);
-                    const uint32_t total = min(s_cnt[warp], (uint32_t)B200PT_PAIR_CAP);
-                    const uint32_t rank = (uint32_t)__popc(act & ((1u << lane) - 1u)), nact = (uint32_t)__popc(act);
-                    for (uint32_t base = 0; base < total; base += nact) {
-                        const uint32_t k = base + rank;
-                        const uint32_t pr = k < total ? wp[k] : 0xffffffffu;
-                        bool hit = false;
-                        unsigned long long key = 0;
-                        TriHit h;
-                        float *col = warp_rays;
-                        uint32_t ti = 0;
-                        if (pr != 0xffffffffu) {
-                            col = warp_rays + (pr >> 27);
-                            ti = pr & 0x7ffffffu;
-                            RayShear sh;
-                            sh.Sx = col[3 * 128];
-                            sh.Sy = col[4 * 128];
-                            sh.Sz = col[5 * 128];
-                            sh.kz = __float_as_int(col[6 * 128]);
-                            sh.kx = sh.kz == 2 ? 0 : sh.kz + 1;
-                            sh.ky = sh.kx == 2 ? 0 : sh.kx + 1;
-                            const F4 *tp = a.tris + (size_t)ti * 3;
-                            const F4 v0 = ld_f4(tp), v1 = ld_f4(tp + 1), v2 = ld_f4(tp + 2);
-                            hit = triangle_test(mk(v0.x, v0.y, v0.z), mk(v1.x, v1.y, v1.z), mk(v2.x, v2.y, v2.z),
-                                                mk(col[0 * 128], col[1 * 128], col[2 * 128]), sh, col[7 * 128], &h);
-                            if (hit) {
-                                key = ((unsigned long long)__float_as_uint(h.t) << 32) | k;
-                                atomicMin(&s_key[(threadIdx.x & ~31) + (pr >> 27)], key);
-                            }
-                        }
-                        __syncwarp(act);
-                        if (hit && s_key[(threadIdx.x & ~31) + (pr >> 27)] == key) {
-                            col[7 * 128] = h.t;  // primitive.cpp:120
-                            col[8 * 128] = __uint_as_float(ti);
-                            col[9 * 128] = h.t;
-                            col[10 * 128] = h.b0;
-                            col[11 * 128] = h.b1;
-                            col[12 * 128] = h.b2;
-                        }
-                        __syncwarp(act);
-                    }
-                    bool was_hit = cnt && !own && s_key[threadIdx.x] != ~0ull;
-                    if (own) {
-                        TravRay R;
-                        ray_load(my_ray, R);
-                        const uint32_t before = R.best;
-                        trav_tri_phase<ANY_HIT, false>(R, a.tri_base, a.tris, pend_x, pend_y, &ctr);
-                        was_hit = R.best != before;
-                        if (was_hit) ray_store_hit(my_ray, R);
-                    }
-                    if (was_hit) {
-                        if (ANY_HIT) {
-                            done = true;
-                        } else {  // the ray got shorter: the box parameter ends at the hit from now on
-                            TravRay R;
-                            ray_load_scale(my_ray, R);
-                            R.tmax = my_ray[7 * 128];
-                            trav_rescale(T, R, R.tmax);
-                        }
-                    }
-                }
-#else
                 if (pend_y) {
                     TravRay R;
                     ray_load(my_ray, R);
@@ -663,25 +474,6 @@ __global__ void __launch_bounds__(128, CTAS) k_trace(const TraceArgs a) {
                         }
                     }
                 }
-#endif
-#if B200PT_PARK_DEPTH > 1
-                // the queue moves up: second -> first, a group found in this step -> second
-                pend_x = my_park[0];
-                pend_y = my_park[128];
-                my_park[0] = ng_x;
-                my_park[128] = ng_y;
-                if (pend_y == 0) {
-                    pend_x = ng_x;
-                    pend_y = ng_y;
-                    my_park[128] = 0;
-                }
-                if (done) {
-                    has = false;
-                    fin = true;
-                    pend_y = 0;
-                    my_park[128] = 0;
-                }
-#else
                 pend_x = ng_x;
                 pend_y = ng_y;
                 if (done) {
@@ -689,7 +481,6 @@ __global__ void __launch_bounds__(128, CTAS) k_trace(const TraceArgs a) {
                     fin = true;
                     pend_y = 0;
                 }
-#endif
             }
             if (has && !trav_next_group(T, S) && pend_y == 0) {
                 has = false;
@@ -2896,66 +2687,6 @@ __global__ void __launch_bounds__(128) k_spatial_cdf(const RenderDev *R) {
     R->sp_func_int[vox] = funcInt;
 }
 
-#if B200PT_NSPEC == 3 && !defined(B200PT_HOST_EMU)  // spectrum-independent (block-synchronous: not in the CPU check build)
-// ------------------------------------------------------------------------ sort
-// Coherence sort between bounces: rays that start in the same cell of a 32^3 grid and travel into
-// the same octant become neighbours in the queue, so the lanes of a warp walk the same top of the
-// tree and touch the same cache lines.  Three small kernels: histogram of keys, exclusive scan,
-// scatter.  Pure integer work on 4-byte records, bound by HBM/L2 bandwidth.
-__device__ __forceinline__ uint32_t spread5(uint32_t v) {  // 5 bits -> every third bit
-    v &= 0x1fu;
-    v = (v | (v << 8)) & 0x100fu;
-    v = (v | (v << 4)) & 0x10c3u;
-    v = (v | (v << 2)) & 0x1249u;
-    return v;
-}
-__device__ __forceinline__ uint32_t coherence_key(const RenderDev *R, const float4 &o, const float4 &d) {
-    const int cx = min(31, max(0, (int)((o.x - R->sort_lo[0]) * R->sort_inv[0])));
-    const int cy = min(31, max(0, (int)((o.y - R->sort_lo[1]) * R->sort_inv[1])));
-    const int cz = min(31, max(0, (int)((o.z - R->sort_lo[2]) * R->sort_inv[2])));
-    const uint32_t oct = (d.x < 0.f ? 1u : 0u) | (d.y < 0.f ? 2u : 0u) | (d.z < 0.f ? 4u : 0u);
-    return (oct << 15) | spread5((uint32_t)cx) | (spread5((uint32_t)cy) << 1) | (spread5((uint32_t)cz) << 2);
-}
-__global__ void __launch_bounds__(256) k_sort_hist(const RenderDev *R, const uint32_t *queue, const uint32_t *count,
-                                                   const float4 *ray_o, const float4 *ray_d) {
-    const uint32_t n = *count;
-    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-        const uint32_t slot = queue[i];
-        const uint32_t key = coherence_key(R, ray_o[(size_t)slot * REC_F4], ray_d[(size_t)slot * REC_F4]);
-        R->sort_keys[i] = key;
-        atomicAdd(&R->sort_hist[key], 1u);
-    }
-}
-__global__ void __launch_bounds__(1024) k_sort_scan(uint32_t *hist) {
-    __shared__ uint32_t partial[1024];
-    const uint32_t per = SORT_BUCKETS / 1024u;
-    uint32_t *mine = hist + threadIdx.x * per;
-    uint32_t sum = 0;
-    for (uint32_t i = 0; i < per; ++i) sum += mine[i];
-    partial[threadIdx.x] = sum;
-    __syncthreads();
-    for (uint32_t off = 1; off < 1024u; off <<= 1) {  // Hillis-Steele inclusive scan
-        uint32_t v = threadIdx.x >= off ? partial[threadIdx.x - off] : 0u;
-        __syncthreads();
-        partial[threadIdx.x] += v;
-        __syncthreads();
-    }
-    uint32_t run = partial[threadIdx.x] - sum;  // exclusive prefix of this thread's segment
-    for (uint32_t i = 0; i < per; ++i) {
-        const uint32_t c = mine[i];
-        mine[i] = run;
-        run += c;
-    }
-}
-__global__ void __launch_bounds__(256) k_sort_scatter(const RenderDev *R, const uint32_t *queue, const uint32_t *count) {
-    const uint32_t n = *count;
-    for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
-        const uint32_t pos = atomicAdd(&R->sort_hist[R->sort_keys[i]], 1u);
-        R->q_sorted[pos] = queue[i];
-    }
-}
-
-#endif  // B200PT_NSPEC == 3
 // ------------------------------------------------------------------------ film
 // One block per tile, one thread per pixel of the tile's FilmTile (the tile
 // plus a one-pixel apron, film.cpp:95-106).  A thread re-creates the
@@ -3210,9 +2941,12 @@ void launch_raygen(const RenderDev *dev, uint32_t batch_first_tile, uint32_t n_b
 }
 
 #if B200PT_NSPEC == 3  // spectrum-independent: compiled once, in the RGBSpectrum translation unit
-#ifdef B200PT_HOST_EMU
 void launch_trace(const TraceArgs &a, bool any_hit, bool classify, bool count, int n_sm, cudaStream_t s) {
-    const int grid = n_sm;
+#ifdef B200PT_HOST_EMU
+    const int grid = n_sm;  // the per-ray k_trace of the check build has no occupancy to fill
+#else
+    const int grid = n_sm * B200PT_TRACE_CTAS;
+#endif
     if (any_hit) {
         if (count)
             B200PT_LAUNCH(B200PT_KERNEL(k_trace<true, false, true>), grid, 128, s, a);
@@ -3230,45 +2964,6 @@ void launch_trace(const TraceArgs &a, bool any_hit, bool classify, bool count, i
             B200PT_LAUNCH(B200PT_KERNEL(k_trace<false, false, false>), grid, 128, s, a);
     }
 }
-#else
-// B200PT_TRACE_VARIANTS (experiment builds): also instantiate the 6- and 8-CTA register budgets and the TMA-staged
-// variant, selectable at run time (TraceArgs::ctas, ::n_staged); the product builds the one configuration that measured best.
-template <bool ANY_HIT, bool CLASSIFY>
-static void launch_trace_variant(const TraceArgs &a, bool count, int n_sm, cudaStream_t s) {
-    if (count) {  // instrumented pass
-        B200PT_LAUNCH(B200PT_KERNEL(k_trace<ANY_HIT, CLASSIFY, true, B200PT_TRACE_CTAS, false>), n_sm * B200PT_TRACE_CTAS, 128, s, a);
-        return;
-    }
-#ifdef B200PT_TRACE_VARIANTS
-    const bool stage = a.n_staged > 0;
-    const size_t smem = stage ? (size_t)a.n_staged * 64 : 0;
-    if (stage) {
-        if (a.ctas == 6)
-            B200PT_LAUNCH_SMEM(B200PT_KERNEL(k_trace<ANY_HIT, CLASSIFY, false, 6, true>), n_sm * 6, 128, smem, s, a);
-        else
-            B200PT_LAUNCH_SMEM(B200PT_KERNEL(k_trace<ANY_HIT, CLASSIFY, false, 8, true>), n_sm * 8, 128, smem, s, a);
-        return;
-    }
-    if (a.ctas == 6) {
-        B200PT_LAUNCH(B200PT_KERNEL(k_trace<ANY_HIT, CLASSIFY, false, 6, false>), n_sm * 6, 128, s, a);
-        return;
-    }
-    if (a.ctas == 8) {
-        B200PT_LAUNCH(B200PT_KERNEL(k_trace<ANY_HIT, CLASSIFY, false, 8, false>), n_sm * 8, 128, s, a);
-        return;
-    }
-#endif
-    B200PT_LAUNCH(B200PT_KERNEL(k_trace<ANY_HIT, CLASSIFY, false, B200PT_TRACE_CTAS, false>), n_sm * B200PT_TRACE_CTAS, 128, s, a);
-}
-void launch_trace(const TraceArgs &a, bool any_hit, bool classify, bool count, int n_sm, cudaStream_t s) {
-    if (any_hit)
-        launch_trace_variant<true, false>(a, count, n_sm, s);
-    else if (classify)
-        launch_trace_variant<false, true>(a, count, n_sm, s);
-    else
-        launch_trace_variant<false, false>(a, count, n_sm, s);
-}
-#endif
 
 #ifndef B200PT_HOST_EMU
 void launch_trace2(const TraceArgs &a, bool any_hit, bool classify, int n_sm, cudaStream_t s) {
@@ -3350,16 +3045,6 @@ void launch_spatial_build(const RenderDev *dev, const RenderDev &host, cudaStrea
     B200PT_LAUNCH(B200PT_KERNEL(k_spatial_cdf), (unsigned)((nvox + 127) / 128), 128, s, dev);
 }
 
-#if B200PT_NSPEC == 3 && !defined(B200PT_HOST_EMU)
-void launch_sort_queue(const RenderDev *dev, const RenderDev &host, const uint32_t *queue, const uint32_t *count,
-                       const float4 *ray_o, const float4 *ray_d, int grid, cudaStream_t s) {
-    cudaMemsetAsync(host.sort_hist, 0, SORT_BUCKETS * sizeof(uint32_t), s);
-    B200PT_LAUNCH(B200PT_KERNEL(k_sort_hist), grid, 256, s, dev, queue, count, ray_o, ray_d);
-    B200PT_LAUNCH(B200PT_KERNEL(k_sort_scan), 1, 1024, s, host.sort_hist);
-    B200PT_LAUNCH(B200PT_KERNEL(k_sort_scatter), grid, 256, s, dev, queue, count);
-}
-
-#endif  // B200PT_NSPEC == 3
 void launch_film(const RenderDev *dev, uint32_t batch_first_tile, uint32_t n_batch_tiles, cudaStream_t s) {
     B200PT_LAUNCH(B200PT_KERNEL(k_film), n_batch_tiles, dim3(18, 18), s, dev, batch_first_tile);
 }

@@ -137,10 +137,6 @@ struct RenderDev {
     uint32_t *q_mat[4];
     uint32_t *q_shadow;
     uint32_t *q_mis;
-    uint32_t *q_sorted;        // queue re-ordered by (ray octant, Morton cell of the origin)
-    uint32_t *sort_keys;       // key per queue entry
-    uint32_t *sort_hist;       // [SORT_BUCKETS] counting-sort histogram / cursors
-    float sort_lo[3], sort_inv[3];  // origin -> 32^3 grid over the scene bounds
     uint32_t *qcount;          // [(max_depth + 2) * Q_PER_BOUNCE]
     uint32_t *work;            // persistent-fetch counters, one per launch of a batch
     unsigned long long *stats; // camera, regular, shadow, nodes, tris
@@ -169,6 +165,7 @@ struct RenderDev {
 
 // resident CTAs of k_trace per SM (128 threads each).  7 (up to 72 registers, no spills) measured fastest on the H100
 // (cfg4, 16 batches, profiles/README.md): +3 % over 8 (64 registers, a few spilled per-ray constants) and +1.5 % over 6.
+// Another count is an A/B build of its own: make VARIANT=ctas8 EXTRA=-DB200PT_TRACE_CTAS=8.
 #ifndef B200PT_TRACE_CTAS
 #define B200PT_TRACE_CTAS 7
 #endif
@@ -197,12 +194,8 @@ struct TraceArgs {
     uint32_t *qcount_mat;  // &qcount[bounce*Q_PER_BOUNCE + Q_MAT0]
     const b200pt_material *materials;
     unsigned long long *stats;  // nodes/tris counters when instrumented
-    int ctas;                   // resident CTAs per SM the launch is compiled for (B200PT_TRACE_CTAS, 6 or 8), 0 = default
-    uint32_t n_staged;          // > 0: k_trace copies nodes [0, n_staged) -- the top of the breadth-first tree -- into shared
-                                // memory with one TMA bulk copy (cp.async.bulk + mbarrier) and reads them there
     int refill_lanes;           // refill the warp when fewer lanes than this are still traversing
     int postpone_pct;           // triangle postponing threshold (% of converged lanes), 0 = off
-    uint32_t magic;             // 0x47000000 as a run-time value (PRMT's second source stays in a register, see plane_2p15)
     // sphere pass (launch_spheres): same rays, after the traversal launch
     const DevSphere *spheres;
     uint32_t n_spheres;
@@ -222,7 +215,7 @@ __device__ __forceinline__ T &slot_out(T *base, uint32_t slot, int stride) {
 
 void launch_raygen(const RenderDev *dev, uint32_t batch_first_tile, uint32_t n_batch_tiles, uint32_t n_slots,
                    cudaStream_t s);
-// grid = SMs of the device (the launcher multiplies by the CTAs per SM of the chosen variant)
+// grid = SMs of the device (the launcher multiplies by B200PT_TRACE_CTAS)
 void launch_trace(const TraceArgs &a, bool any_hit, bool classify, bool count, int n_sm, cudaStream_t s);
 // Scenes with object instances (and a tree over them): top-level triangles + instances in one persistent two-level
 // traversal (k_trace2); launch_spheres is then only needed for Sphere shapes.  Not part of the CPU check build.
@@ -245,12 +238,6 @@ void launch_medium_general(const RenderDev *dev, const RenderDev &host, int boun
 // ray (occluded / A or mis_hit / B final) or re-queues it behind the boundary into q_walk[out] / *walk_count.
 void launch_direct_walk(const RenderDev *dev, const RenderDev &host, bool shadow, const uint32_t *queue, const uint32_t *count,
                         int out, uint32_t *walk_count, uint32_t *work, bool count_rays, int grid, cudaStream_t s);
-#define SORT_BUCKETS (1u << 18)  // 3 octant bits + 15 Morton bits
-// Counting sort of a queue of slots by the coherence key of the rays they refer to; `out` receives
-// the permuted queue (order inside a bucket is arbitrary -- it never affects a path's arithmetic).
-// ray_o / ray_d point at the ray pair of slot 0 in the per-slot records (stride REC_F4).
-void launch_sort_queue(const RenderDev *dev, const RenderDev &host, const uint32_t *queue, const uint32_t *count,
-                       const float4 *ray_o, const float4 *ray_d, int grid, cudaStream_t s);
 void launch_sobol_table(const uint32_t *mat32, uint32_t *table, int n_dims, cudaStream_t s);
 // Fills the per-voxel light distributions (all voxels, once per render object).
 void launch_spatial_build(const RenderDev *dev, const RenderDev &host, cudaStream_t s);

@@ -385,7 +385,7 @@ B200_HD void lbvh_collapse(const LbvhCtx &c, const LbvhItem &it) {
         }
     }
     if (it.wide < c.node_cap) {
-        wbvh_store_node(c.nodes, it.wide, node);
+        memcpy(&c.nodes[it.wide], &node, sizeof(node));  // as bytes: an assignment costs k_lbvh_collapse 4 registers
         c.tri_base[it.wide] = triBase;
     }
 }

@@ -26,7 +26,6 @@
     ::b200pt_emu::launch(dim3(grid), dim3(block), [&]() { kernel(__VA_ARGS__); })
 #else
 #define B200PT_LAUNCH(kernel, grid, block, stream, ...) kernel<<<(grid), (block), 0, (stream)>>>(__VA_ARGS__)
-#define B200PT_LAUNCH_SMEM(kernel, grid, block, smem, stream, ...) kernel<<<(grid), (block), (smem), (stream)>>>(__VA_ARGS__)
 #endif
 
 #ifdef __CUDACC__

@@ -45,12 +45,6 @@ namespace b200pt {
 #define B200PT_WIDTH 7          // children per node
 #define B200PT_EMPTY_LO 255u    // quantised box of an empty slot: lo > hi
 #define B200PT_CELL_FLOOR 0x1p-17f  // smallest cell, relative to the largest |coordinate| of the tree (see wbvh_traverse.cuh)
-// Storage order of a record's two 32-byte halves (experiment, off): with B200PT_NODE_SWIZZLE node i is stored with its
-// halves swapped when bit 1 of i is set, so that the first load of a warp's lanes -- different nodes, same
-// instruction -- spreads over more of L1's data banks.  It made no measurable difference, so records are stored as they are.
-#ifndef B200PT_NODE_SWIZZLE
-#define B200PT_NODE_SWIZZLE 0
-#endif
 
 struct alignas(64) WbvhNode {
     float p[3];
@@ -96,9 +90,6 @@ B200_HD float wb_u2f(uint32_t u) {
 #endif
 }
 B200_HD float wb_cell(uint8_t e) { return wb_u2f((uint32_t)e << 23); }
-
-// 1 if node `index` (counted from the root of its own tree) is stored with swapped halves
-B200_HD uint32_t wb_swapped(uint32_t index) { return B200PT_NODE_SWIZZLE ? ((index >> 1) & 1u) : 0u; }
 
 // Octant-ordered slot assignment (greedy on dot(centroid offset, octant direction)): visiting the slots by
 // (slot XOR ray octant), highest first, then approximates front-to-back order.  childAt[s] = child or -1.
@@ -209,27 +200,9 @@ B200_HD void wbvh_encode_node(const WbBox *box, const int *childAt, const uint8_
     }
 }
 
-// node record <-> storage order (byte copies: no type punning)
-B200_HD void wbvh_store_node(WbvhNode *array, uint32_t index, const WbvhNode &n) {
-    const unsigned char *src = reinterpret_cast<const unsigned char *>(&n);
-    unsigned char *dst = reinterpret_cast<unsigned char *>(array + index);
-    const uint32_t r = wb_swapped(index) * 32u;
-    memcpy(dst, src + r, 32);
-    memcpy(dst + 32, src + (32u - r), 32);
-}
-B200_HD WbvhNode wbvh_load_node(const WbvhNode *array, uint32_t index) {
-    WbvhNode n;
-    const unsigned char *src = reinterpret_cast<const unsigned char *>(array + index);
-    unsigned char *dst = reinterpret_cast<unsigned char *>(&n);
-    const uint32_t r = wb_swapped(index) * 32u;
-    memcpy(dst, src + r, 32);
-    memcpy(dst + 32, src + (32u - r), 32);
-    return n;
-}
-
 #ifndef __CUDACC_RTC__
 struct Wbvh {
-    std::vector<WbvhNode> nodes;     // node 0 is the root; records in STORAGE order (wbvh_store_node / wbvh_load_node)
+    std::vector<WbvhNode> nodes;     // node 0 is the root
     std::vector<uint32_t> tri_base;  // per node: first triangle of its leaf children
     std::vector<TriRecord> tris;     // leaf order; degenerate triangles (never hittable) at the end
     std::vector<uint32_t> prim_to_tri;  // original triangle index -> position in `tris`

@@ -376,7 +376,7 @@ void build_wbvh(const float *vertices, int64_t n_tris, const int32_t *material_i
                     out->nodes.push_back(WbvhNode());
                 }
             }
-            wbvh_store_node(out->nodes.data(), cur.wide, node);
+            out->nodes[cur.wide] = node;
             if (out->tri_base.size() < out->nodes.size()) out->tri_base.resize(out->nodes.size(), 0u);
             out->tri_base[cur.wide] = triBase;
         }
@@ -424,7 +424,7 @@ int64_t validate_wbvh(const Wbvh &bvh) {
     // true content bounds bottom-up (children have larger indices than their parents)
     std::vector<Box> content(bvh.nodes.size());
     for (int64_t ni = (int64_t)bvh.nodes.size() - 1; ni >= 0; --ni) {
-        const WbvhNode n = wbvh_load_node(bvh.nodes.data(), (uint32_t)ni);
+        const WbvhNode &n = bvh.nodes[ni];
         Box cb;
         cb.reset();
         uint32_t inner = 0, triOff = 0;

@@ -72,26 +72,11 @@ B200_D F4 ld_f4(const F4 *p) {
     return r;
 }
 // one 64-byte node = four 128-bit loads (LDG.E.128.CONSTANT; sm_90 has no 256-bit global load)
-// (the first two fetch the record's logical first half wherever the storage order put it, see wbvh.h)
 B200_D void ld_node(const U4 *nodes, uint32_t index, NodeWords *n) {
     const uint8_t *p = reinterpret_cast<const uint8_t *>(nodes) + (size_t)index * 64;
-    const uint32_t r = b200pt::wb_swapped(index) << 5;
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
-        const uint4 v = __ldg(reinterpret_cast<const uint4 *>(p + ((r ^ (uint32_t)(j >> 1) * 32u) + (uint32_t)(j & 1) * 16u)));
-        n->w[4 * j] = v.x;
-        n->w[4 * j + 1] = v.y;
-        n->w[4 * j + 2] = v.z;
-        n->w[4 * j + 3] = v.w;
-    }
-}
-// the same record from the CTA's shared-memory copy of the top of the tree (k_trace's TMA-staged variant)
-B200_D void ld_node_smem(const U4 *staged, uint32_t index, NodeWords *n) {
-    const uint4 *p = reinterpret_cast<const uint4 *>(staged) + (size_t)index * 4;
-    const uint32_t r = b200pt::wb_swapped(index) << 1;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) {
-        const uint4 v = p[j ^ r];
+        const uint4 v = __ldg(reinterpret_cast<const uint4 *>(p + 16 * j));
         n->w[4 * j] = v.x;
         n->w[4 * j + 1] = v.y;
         n->w[4 * j + 2] = v.z;
@@ -126,11 +111,7 @@ B200_D int popc32(uint32_t v) { return __popc(v); }
 #else
 inline U4 ld_u4(const U4 *p) { return *p; }
 inline F4 ld_f4(const F4 *p) { return *p; }
-inline void ld_node(const U4 *nodes, uint32_t index, NodeWords *n) {
-    const b200pt::WbvhNode rec = b200pt::wbvh_load_node(reinterpret_cast<const b200pt::WbvhNode *>(nodes), index);
-    memcpy(n->w, &rec, 64);
-}
-inline void ld_node_smem(const U4 *staged, uint32_t index, NodeWords *n) { ld_node(staged, index, n); }
+inline void ld_node(const U4 *nodes, uint32_t index, NodeWords *n) { memcpy(n->w, nodes + (size_t)index * 4, 64); }
 inline float fma_any(float a, float b, float c) { return fmaf(a, b, c); }
 inline float fma_sat(float a, float b, float c) {
     const float r = fmaf(a, b, c);
@@ -300,12 +281,9 @@ B200_HD void trav_init(Trav &T, TravRay &R, const V3 &o, const V3 &d, float rayT
 // leaf group (*tg_x = the node, *tg_y = hit leaf slots | lcount << 8, 0 if none).  Requires T.cur to be a node group.
 // (CLOSEST is kept for the callers' sake: a closest hit rescales the box parameter, trav_rescale, so the test itself is
 // the same for both kinds of ray.)
-// STAGE: nodes [0, n_staged) -- the top of the tree, which is stored breadth-first -- are read from `staged`, a copy in
-// shared memory, instead of global memory.
-template <bool CLOSEST, bool COUNT, bool STAGE = false, class Stack = TravStack>
-B200_HD void trav_node_phase(Trav &T, Stack &S, const U4 *__restrict__ nodes, const uint32_t *__restrict__ /*tri_base*/,
-                             const uint8_t *lut, uint32_t *tg_x, uint32_t *tg_y, TraceCounters *ctr, const U4 *staged = nullptr,
-                             uint32_t n_staged = 0) {
+template <bool CLOSEST, bool COUNT>
+B200_HD void trav_node_phase(Trav &T, TravStack &S, const U4 *__restrict__ nodes, const uint32_t *__restrict__ /*tri_base*/,
+                             const uint8_t *lut, uint32_t *tg_x, uint32_t *tg_y, TraceCounters *ctr) {
     const uint32_t hits = T.cur_y;
     const int bit = msb32(hits);
     T.cur_y &= ~(1u << bit);
@@ -321,10 +299,7 @@ B200_HD void trav_node_phase(Trav &T, Stack &S, const U4 *__restrict__ nodes, co
     const uint32_t rel = (uint32_t)popc32(hits & 0xffu & ((1u << slot) - 1u));
     const uint32_t ni = T.cur_x + rel;
     NodeWords n;
-    if (STAGE && ni < n_staged)
-        ld_node_smem(staged, ni, &n);
-    else
-        ld_node(nodes, ni, &n);
+    ld_node(nodes, ni, &n);
     if (COUNT) ctr->nodes++;
     // w0-2: p   w3: e.x e.y e.z imask   w4: child_base   w5: lcount | z pair of slot 0   w6-8: z pairs of slots 1..6
     // w9+s: (lo.x hi.x lo.y hi.y) of slot s.  plane(q) = p + q*cell, in box-parameter units q*a + k with a = cell/d,
@@ -359,19 +334,6 @@ B200_HD void trav_node_phase(Trav &T, Stack &S, const U4 *__restrict__ nodes, co
 #endif
     T.cur_x = n.w[4];
     T.cur_y = (pm << 24) | imask;
-#if defined(__CUDA_ARCH__) && defined(B200PT_PREFETCH_CHILDREN)
-    {   // experiment: the hit children that will wait on the stack (all but the first in traversal order) are pulled
-        // into L2 now, so that their fetch -- many steps later -- does not go to DRAM
-        uint32_t rest = pm & (pm - 1u) ? pm & ~(1u << msb32(pm)) : 0u;
-        while (rest) {
-            const int b = msb32(rest);
-            rest &= ~(1u << b);
-            const uint32_t sl = (uint32_t)b ^ T.octinv;
-            const uint32_t ci = n.w[4] + (uint32_t)popc32(imask & ((1u << sl) - 1u));
-            asm volatile("prefetch.global.L2 [%0];" ::"l"(reinterpret_cast<const uint8_t *>(nodes) + (size_t)ci * 64));
-        }
-    }
-#endif
     // leaf children that were hit: the node's number and (slot bits | lcount << 8); trav_tri_phase turns them into triangles
     const uint32_t ml = m & ~imask;
     *tg_x = ni;
@@ -423,8 +385,7 @@ B200_HD bool trav_tri_phase(TravRay &R, const uint32_t *__restrict__ tri_base, c
 }
 
 // Pops the next node group if the current one is exhausted; false when nothing is left.
-template <class Stack>
-B200_HD bool trav_next_group(Trav &T, Stack &S) {
+B200_HD bool trav_next_group(Trav &T, TravStack &S) {
     if ((T.cur_y & 0xff000000u) == 0) {
         if ((T.sp & B200PT_SP_MASK) == 0) return false;
         --T.sp;

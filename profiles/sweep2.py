@@ -1,5 +1,5 @@
 """Round-2 knob sweep on one scene build: times a few wavefront batches of a workload for each k_trace setting
-(b200pt_render_set_option: trace_ctas, stage_nodes, refill_lanes, postpone_pct).  Device time per kernel class comes
+(b200pt_render_set_option: refill_lanes, postpone_pct, overlap).  Device time per kernel class comes
 from the library's own CUDA events ("profile"); rays are the reference's counters.
 
   python profiles/sweep2.py [workload] [n_batches] [setting ...]     setting = name=value[,name=value...]
@@ -17,8 +17,7 @@ import bench  # noqa: E402
 
 name = sys.argv[1] if len(sys.argv) > 1 else "cfg3"
 n_batches = int(sys.argv[2]) if len(sys.argv) > 2 else 3
-settings = sys.argv[3:] or ["", "trace_ctas=8", "stage_nodes=57", "stage_nodes=400", "trace_ctas=8,stage_nodes=57",
-                            "refill_lanes=22", "refill_lanes=28", "postpone_pct=25", "postpone_pct=60", "overlap=0"]
+settings = sys.argv[3:] or ["", "refill_lanes=22", "refill_lanes=28", "postpone_pct=25", "postpone_pct=60", "overlap=0"]
 pkg = graft.load_package()
 from pbrt_v3_distributed_b200 import scenes  # noqa: E402
 
@@ -38,7 +37,7 @@ r = pkg.Render(scene, setup)
 per_batch = max(1, int(os.environ.get("B200PT_BATCH_PATHS", 16 << 20)) // (256 * spp))
 mid = (r.tiles_y // 2) * r.tiles_x + r.tiles_x // 4
 tiles = (mid + np.arange(per_batch * n_batches)) % r.n_tiles
-defaults = dict(trace_ctas=0, stage_nodes=0, refill_lanes=26, postpone_pct=40, overlap=1)
+defaults = dict(refill_lanes=26, postpone_pct=40, overlap=1)
 # instrumented pass once: nodes / triangles per ray
 r.set_option("instrument", 1)
 r.render_tiles(tiles[:per_batch])

@@ -12,12 +12,3 @@ bool build_wbvh_gpu(const GpuBuildInput &, cudaStream_t, GpuBuildOutput *, char 
 }
 }  // namespace b200pt
 
-// The coherence sort of the ray queues (off by default, B200PT_SORT_FROM) is a block-synchronous scan.
-#include "kernels.cuh"
-namespace b200pt {
-void launch_sort_queue(const RenderDev *, const RenderDev &, const uint32_t *, const uint32_t *, const float4 *, const float4 *, int,
-                       cudaStream_t) {
-    fprintf(stderr, "the queue sort is not part of the CPU check build\n");
-    abort();
-}
-}  // namespace b200pt
