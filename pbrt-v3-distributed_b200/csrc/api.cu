@@ -101,7 +101,7 @@ struct b200pt_render {
     int32_t *d_tile_list = nullptr;
     size_t tile_list_capacity = 0;
     float *d_rgb = nullptr;  // b200pt_film_read_rgb staging (lazily allocated, freed with the render object)
-    uint32_t *d_walk_counts = nullptr;  // bounded media: [16] queue counters / fetch counters of the boundary passes
+    uint32_t *d_walk_counts = nullptr;  // bounded media: [WC_COUNT] queue counters / fetch counters of the boundary passes
     int grid_trace = 0, grid_shade = 0, grid_shade_s60 = 0;
     bool instrumented = false, profiling = false;
     int refill_lanes = 26, postpone_pct = 40;  // k_trace knobs (b200pt_render_set_option)
@@ -377,7 +377,7 @@ int b200pt_scene_create(b200pt_ctx *ctx, const b200pt_scene_desc *d, b200pt_scen
         obj_bounds[o] = make_trav_bounds(ob.bounds_lo, ob.bounds_hi);
         for (TriRecord t : ob.tris) {
             t.prim += (uint32_t)first;      // back to the scene's triangle numbering
-            t.mat_flags |= 0x100000u;       // object-space triangle: shading goes through the instance transform
+            t.mat_flags |= B200PT_TRI_INSTANCED;  // object-space triangle: shading goes through the instance transform
             bvh.tris.push_back(t);
         }
         for (int64_t i = 0; i < count; ++i) bvh.prim_to_tri[(size_t)(first + i)] = obj_tri_off[o] + ob.prim_to_tri[(size_t)i];
@@ -392,7 +392,7 @@ int b200pt_scene_create(b200pt_ctx *ctx, const b200pt_scene_desc *d, b200pt_scen
             memcpy(t.p1, v + 3, 12);
             memcpy(t.p2, v + 6, 12);
             t.prim = (uint32_t)i;
-            t.mat_flags = (uint32_t)d->material_id[i] | 0x20000u | 0x100000u;
+            t.mat_flags = (uint32_t)d->material_id[i] | B200PT_TRI_DEGENERATE | B200PT_TRI_INSTANCED;
             t.light = -1;
             bvh.prim_to_tri[(size_t)i] = (uint32_t)bvh.tris.size();
             bvh.tris.push_back(t);
@@ -475,13 +475,13 @@ int b200pt_scene_create(b200pt_ctx *ctx, const b200pt_scene_desc *d, b200pt_scen
         if (d->normals && (vf & 1)) {
             const float *n = d->normals + 9 * i;
             for (int k = 0; k < 3; ++k) tri_n[(size_t)ti * 3 + k] = F4{n[3 * k], n[3 * k + 1], n[3 * k + 2], 0.f};
-            if (!gpu_build) bvh.tris[ti].mat_flags |= 0x40000u;  // the device builder sets the flags itself
+            if (!gpu_build) bvh.tris[ti].mat_flags |= B200PT_TRI_HAS_NORMALS;  // the device builder sets the flags itself
         }
         if (d->uvs && (vf & 2)) {
             const float *u = d->uvs + 6 * i;
             tri_uv[(size_t)ti * 2] = F4{u[0], u[1], u[2], u[3]};
             tri_uv[(size_t)ti * 2 + 1] = F4{u[4], u[5], 0.f, 0.f};
-            if (!gpu_build) bvh.tris[ti].mat_flags |= 0x80000u;
+            if (!gpu_build) bvh.tris[ti].mat_flags |= B200PT_TRI_HAS_UVS;
         }
     }
 
@@ -537,7 +537,7 @@ int b200pt_scene_create(b200pt_ctx *ctx, const b200pt_scene_desc *d, b200pt_scen
         sp.z_max = zMax;
         sp.area = sp.phi_max * r * (zMax - zMin);
         const bool flip = (in.reverse_orientation != 0) ^ (in.transform_swaps_handedness != 0);
-        sp.mat_flags = (uint32_t)in.material_id | (flip ? 0x10000u : 0u);
+        sp.mat_flags = (uint32_t)in.material_id | (flip ? B200PT_TRI_FLIP : 0u);
         sp.light_id = in.light_id;
         sp.reverse_orientation = in.reverse_orientation != 0;
         // Shape::WorldBound (shape.cpp:52, transform.cpp:246-256) joins Scene::WorldBound()
@@ -1191,7 +1191,7 @@ int b200pt_render_create(b200pt_scene *scene, const b200pt_camera_desc *cam, con
     ALLOC(H.q_shadow, cap);
     ALLOC(H.q_mis, cap);
     ALLOC(H.qcount, (size_t)(H.max_depth + 2) * Q_PER_BOUNCE);
-    ALLOC(H.work, (size_t)(H.max_depth + 2) * 16);
+    ALLOC(H.work, (size_t)(H.max_depth + 2) * W_PER_BOUNCE);
     ALLOC(H.stats, 9);
     // media bounded by surfaces: medium table, per-sphere medium ids, the walkers' per-slot state
     float *d_media_tab = nullptr, *d_media_g = nullptr;
@@ -1228,7 +1228,7 @@ int b200pt_render_create(b200pt_scene *scene, const b200pt_camera_desc *cam, con
         ALLOC(H.sh_p1, cap);
         ALLOC(H.sh_p1e, cap);
         ALLOC(H.sh_p1n, cap);
-        ALLOC(r->d_walk_counts, 16);
+        ALLOC(r->d_walk_counts, WC_COUNT);
     }
     ALLOC(r->d_dev, 1);
 #undef ALLOC
@@ -1389,6 +1389,23 @@ static void drain_timers(b200pt_render *r) {
     r->timed.clear();
 }
 
+// One launcher of the spectrum build the scene was made for: inside the argument list `dev` and `host` are the render's
+// device and host RenderDev as that build sees them.
+#define LAUNCH_SPEC(fn, ...)                     \
+    do {                                         \
+        if (spectral) {                          \
+            const auto *dev = s60(r->d_dev);     \
+            const auto &host = s60(r->host);     \
+            (void)host;                          \
+            b200pt_s60::fn(__VA_ARGS__);         \
+        } else {                                 \
+            const RenderDev *dev = r->d_dev;     \
+            const RenderDev &host = r->host;     \
+            (void)host;                          \
+            fn(__VA_ARGS__);                     \
+        }                                        \
+    } while (0)
+
 int b200pt_render_tiles(b200pt_render *r, const int32_t *tiles, int64_t n_tiles) {
     if (!r) return b200pt_fail(B200PT_ERR_INVALID, "render is NULL");
     const int64_t total = (int64_t)r->host.tiles_x * r->host.tiles_y;
@@ -1420,7 +1437,7 @@ int b200pt_render_tiles(b200pt_render *r, const int32_t *tiles, int64_t n_tiles)
     const bool spectral = r->scene->nspec != 0;
     const int maxDepth = H.max_depth;
     const size_t qbytes = (size_t)(maxDepth + 2) * Q_PER_BOUNCE * sizeof(uint32_t);
-    const size_t wbytes = (size_t)(maxDepth + 2) * 16 * sizeof(uint32_t);
+    const size_t wbytes = (size_t)(maxDepth + 2) * W_PER_BOUNCE * sizeof(uint32_t);
     bool families[4] = {false, false, false, false};
     for (const auto &m : r->scene->materials) families[m.type] = true;
 
@@ -1432,10 +1449,7 @@ int b200pt_render_tiles(b200pt_render *r, const int32_t *tiles, int64_t n_tiles)
         CUDA_TRY(cudaMemsetAsync(H.pix_bleed, 0, (size_t)nb * 256, st));
         {
             LaunchTimer lt(r, st, 2);
-            if (spectral)
-                b200pt_s60::launch_raygen(s60(r->d_dev), (uint32_t)first, nb, n_slots, st);
-            else
-                launch_raygen(r->d_dev, (uint32_t)first, nb, n_slots, st);
+            LAUNCH_SPEC(launch_raygen, dev, (uint32_t)first, nb, n_slots, st);
         }
         // Launch order per bounce b (path.cpp:81-188):
         //   closest(b) -> shade(b) -> { any(b), MIS-closest(b) } || closest(b+1) -> resolve(b) -> shade(b+1) ...
@@ -1443,7 +1457,7 @@ int b200pt_render_tiles(b200pt_render *r, const int32_t *tiles, int64_t n_tiles)
         // two streams: as the persistent CTAs of one launch drain, the other launch fills the freed SMs.
         const bool general = H.med_general != 0;  // media bounded by surfaces: boundary passes inside a bounce (see RenderDev)
         const bool medium = H.has_medium != 0 || general;  // k_medium also queues direct-lighting rays: no overlap of bounces then
-        uint32_t *const wc = r->d_walk_counts;  // [0], [1] crossers of a pass (ping-pong), [2] walk kernel, [3] trace, [4] sphere pass
+        uint32_t *const wc = r->d_walk_counts;  // the WC_* counters
         auto device_count = [&](const uint32_t *d, cudaStream_t s_) {
             uint32_t v = 0;
             if (cudaMemcpyAsync(&v, d, sizeof(v), cudaMemcpyDeviceToHost, s_) != cudaSuccess) return 0u;
@@ -1471,7 +1485,12 @@ int b200pt_render_tiles(b200pt_render *r, const int32_t *tiles, int64_t n_tiles)
 #endif
             launch_trace(a, any_hit, classify, r->instrumented, r->grid_trace, s_);
         };
-        auto sphere_args = [&](TraceArgs &a, uint32_t *work) {
+        // Scene::Intersect / IntersectP of the ray queue in `a`: the traversal launch and, with `spheres`, the pass over the
+        // shapes outside the tree (fetch counter sphere_work).  With `classify` the hits go to their BSDF family's queue:
+        // by the sphere pass when it runs, since it decides the final hit.
+        auto intersect = [&](TraceArgs &a, bool any_hit, bool classify, bool spheres, uint32_t *sphere_work, cudaStream_t s_) {
+            trace(a, any_hit, classify && !spheres, s_);
+            if (!spheres) return;
             a.sphere_refill_lanes = sphere_refill_lanes();
             a.spheres = H.scene.spheres;
             a.n_spheres = H.scene.n_spheres;
@@ -1481,11 +1500,13 @@ int b200pt_render_tiles(b200pt_render *r, const int32_t *tiles, int64_t n_tiles)
             a.tlas_tri_off = H.scene.tlas_tri_off;
             a.hit_inst_out = a.hit_out == &H.path->hit ? &H.path->hit_inst : nullptr;
             a.n_tris = (uint32_t)r->scene->n_prims;
-            a.sphere_work = work;
+            a.sphere_work = sphere_work;
+            launch_spheres(a, any_hit, classify, r->grid_shade, s_);
+            r->launches++;
         };
         auto trace_path = [&](int b) {
             uint32_t *qc = H.qcount + (size_t)b * Q_PER_BOUNCE;
-            uint32_t *wk = H.work + (size_t)b * 16;
+            uint32_t *wk = H.work + (size_t)b * W_PER_BOUNCE;
             TraceArgs a = trace_args_render(r);
             a.out_stride = (int)sizeof(PathRec);
             // closest hit of the path rays + classification by BSDF family
@@ -1493,7 +1514,7 @@ int b200pt_render_tiles(b200pt_render *r, const int32_t *tiles, int64_t n_tiles)
             a.ray_d = &H.path->d;
             a.queue = H.q_path[b & 1];
             a.count = qc + Q_PATH;
-            a.work = wk + 0;
+            a.work = wk + W_TRACE_PATH;
             a.fixed_t_max = INFINITY;
             a.hit_out = &H.path->hit;
             for (int m = 0; m < 4; ++m) a.q_mat[m] = H.q_mat[m];
@@ -1502,52 +1523,41 @@ int b200pt_render_tiles(b200pt_render *r, const int32_t *tiles, int64_t n_tiles)
                 // closest_ms = the traversal launch and, for scenes with spheres, the pass that completes Scene::Intersect;
                 // the medium pass below is timed on its own (category 2)
                 LaunchTimer lt(r, st, 0);
-                // with spheres in the scene the sphere pass decides the final hit, so it does the classification;
-                // inside a medium the medium pass does (only paths that reach their surface are shaded)
-                trace(a, false, !has_spheres && !medium, st);
-                if (has_spheres) {
-                    sphere_args(a, wk + 8);
-                    launch_spheres(a, false, !medium, r->grid_shade, st);
-                    r->launches++;
-                }
+                // inside a medium the medium pass classifies (only paths that reach their surface are shaded)
+                intersect(a, false, !medium, has_spheres, wk + W_SPHERES_PATH, st);
             }
             if (general) {
                 // the medium pass, then -- while some rays reached a medium boundary -- the same two steps again for those
                 // rays from behind the boundary (volpath.cpp:115-121: no bounce is spent)
-                cudaMemsetAsync(wc, 0, 16 * sizeof(uint32_t), st);
+                cudaMemsetAsync(wc, 0, WC_COUNT * sizeof(uint32_t), st);
                 {
                     LaunchTimer lt2(r, st, 2);
-                    launch_medium_general(r->d_dev, H, b, a.queue, qc + Q_PATH, 0, wc + 0, wk + 11, false, r->grid_shade, st);
+                    launch_medium_general(r->d_dev, H, b, a.queue, qc + Q_PATH, 0, wc + WC_CROSS0, wk + W_MEDIUM, false, r->grid_shade, st);
                 }
                 for (int cur = 0; device_count(wc + cur, st) != 0; cur ^= 1) {
                     cudaMemsetAsync(wc + (cur ^ 1), 0, sizeof(uint32_t), st);
-                    cudaMemsetAsync(wc + 2, 0, 3 * sizeof(uint32_t), st);
+                    cudaMemsetAsync(wc + WC_WALK, 0, 3 * sizeof(uint32_t), st);
                     a.queue = H.q_cross[cur];
                     a.count = wc + cur;
-                    a.work = wc + 3;
+                    a.work = wc + WC_TRACE;
                     {
                         LaunchTimer lt(r, st, 0);
-                        trace(a, false, false, st);
-                        sphere_args(a, wc + 4);
-                        launch_spheres(a, false, false, r->grid_shade, st);
-                        r->launches++;
+                        intersect(a, false, false, true, wc + WC_SPHERES, st);
                     }
                     LaunchTimer lt2(r, st, 2);
-                    launch_medium_general(r->d_dev, H, b, H.q_cross[cur], wc + cur, cur ^ 1, wc + (cur ^ 1), wc + 2, true, r->grid_shade, st);
+                    launch_medium_general(r->d_dev, H, b, H.q_cross[cur], wc + cur, cur ^ 1, wc + (cur ^ 1), wc + WC_WALK, true, r->grid_shade,
+                                          st);
                 }
             } else if (medium) {
                 LaunchTimer lt2(r, st, 2);
-                if (spectral)
-                    b200pt_s60::launch_medium(s60(r->d_dev), b, wk + 11, r->grid_shade, st);
-                else
-                    launch_medium(r->d_dev, b, wk + 11, r->grid_shade, st);
+                LAUNCH_SPEC(launch_medium, dev, b, wk + W_MEDIUM, r->grid_shade, st);
             }
         };
         // Bounded media: the shadow (VisibilityTester::Tr) or MIS (Scene::IntersectTr) rays of bounce b walk from boundary to
         // boundary -- a closest-hit launch per segment, then k_direct_walk ends each ray or sends it on
         auto walk_direct = [&](int b, bool shadow) {
             uint32_t *qc = H.qcount + (size_t)b * Q_PER_BOUNCE;
-            uint32_t *wk = H.work + (size_t)b * 16;
+            uint32_t *wk = H.work + (size_t)b * W_PER_BOUNCE;
             TraceArgs a = trace_args_render(r);
             a.ray_o = shadow ? &H.direct->sh_o : &H.direct->mi_o;
             a.ray_d = shadow ? &H.direct->sh_d : &H.direct->mi_d;
@@ -1556,30 +1566,28 @@ int b200pt_render_tiles(b200pt_render *r, const int32_t *tiles, int64_t n_tiles)
             a.out_stride = shadow ? (int)sizeof(uint32_t) : (int)sizeof(DirectRec);
             const uint32_t *queue = shadow ? H.q_shadow : H.q_mis;
             const uint32_t *count = qc + (shadow ? Q_SHADOW : Q_MIS);
-            uint32_t *trace_work = wk + (shadow ? 5 : 6), *sphere_work = wk + (shadow ? 9 : 10);
-            cudaMemsetAsync(wc, 0, 16 * sizeof(uint32_t), st);
+            uint32_t *trace_work = wk + (shadow ? W_TRACE_SHADOW : W_TRACE_MIS);
+            uint32_t *sphere_work = wk + (shadow ? W_SPHERES_SHADOW : W_SPHERES_MIS);
+            cudaMemsetAsync(wc, 0, WC_COUNT * sizeof(uint32_t), st);
             bool first = true;
             for (int cur = 0;; cur ^= 1) {
                 if (!first) {
                     if (device_count(count, st) == 0) break;
                     cudaMemsetAsync(wc + cur, 0, sizeof(uint32_t), st);
-                    cudaMemsetAsync(wc + 2, 0, 3 * sizeof(uint32_t), st);
-                    trace_work = wc + 3;
-                    sphere_work = wc + 4;
+                    cudaMemsetAsync(wc + WC_WALK, 0, 3 * sizeof(uint32_t), st);
+                    trace_work = wc + WC_TRACE;
+                    sphere_work = wc + WC_SPHERES;
                 }
                 a.queue = queue;
                 a.count = count;
                 a.work = trace_work;
                 {
                     LaunchTimer lt(r, st, 0);
-                    trace(a, false, false, st);
-                    sphere_args(a, sphere_work);
-                    launch_spheres(a, false, false, r->grid_shade, st);
-                    r->launches++;
+                    intersect(a, false, false, true, sphere_work, st);
                 }
                 {
                     LaunchTimer lt2(r, st, 2);
-                    launch_direct_walk(r->d_dev, H, shadow, queue, count, cur, wc + cur, wc + 2, !first, r->grid_shade, st);
+                    launch_direct_walk(r->d_dev, H, shadow, queue, count, cur, wc + cur, wc + WC_WALK, !first, r->grid_shade, st);
                 }
                 queue = H.q_walk[cur];
                 count = wc + cur;
@@ -1593,7 +1601,7 @@ int b200pt_render_tiles(b200pt_render *r, const int32_t *tiles, int64_t n_tiles)
                 return;
             }
             uint32_t *qc = H.qcount + (size_t)b * Q_PER_BOUNCE;
-            uint32_t *wk = H.work + (size_t)b * 16;
+            uint32_t *wk = H.work + (size_t)b * W_PER_BOUNCE;
             TraceArgs a = trace_args_render(r);
             a.out_stride = (int)sizeof(DirectRec);
             // shadow rays (any hit), tMax = 1 - ShadowEpsilon
@@ -1601,55 +1609,39 @@ int b200pt_render_tiles(b200pt_render *r, const int32_t *tiles, int64_t n_tiles)
             a.ray_d = &H.direct->sh_d;
             a.queue = H.q_shadow;
             a.count = qc + Q_SHADOW;
-            a.work = wk + 5;
+            a.work = wk + W_TRACE_SHADOW;
             a.fixed_t_max = PT_SHADOW_TMAX;
             a.occ_out = &H.direct->occluded;
             {
                 LaunchTimer lt(r, st2, 1);
-                trace(a, true, false, st2);
-                if (has_spheres) {
-                    sphere_args(a, wk + 9);
-                    launch_spheres(a, true, false, r->grid_shade, st2);
-                    r->launches++;
-                }
+                intersect(a, true, false, has_spheres, wk + W_SPHERES_SHADOW, st2);
             }
             // BSDF-sampled MIS rays (closest hit)
             a.ray_o = &H.direct->mi_o;
             a.ray_d = &H.direct->mi_d;
             a.queue = H.q_mis;
             a.count = qc + Q_MIS;
-            a.work = wk + 6;
+            a.work = wk + W_TRACE_MIS;
             a.fixed_t_max = INFINITY;
             a.hit_out = &H.direct->mis_hit;
             a.occ_out = nullptr;
             LaunchTimer lt(r, st2, 0);
-            trace(a, false, false, st2);
-            if (has_spheres) {
-                sphere_args(a, wk + 10);
-                launch_spheres(a, false, false, r->grid_shade, st2);
-                r->launches++;
-            }
+            intersect(a, false, false, has_spheres, wk + W_SPHERES_MIS, st2);
         };
         trace_path(0);
         for (int b = 0; b <= maxDepth; ++b) {
-            uint32_t *wk = H.work + (size_t)b * 16;
+            uint32_t *wk = H.work + (size_t)b * W_PER_BOUNCE;
             for (int m = 0; m < 4; ++m)
                 if (families[m]) {
                     LaunchTimer lt(r, st, 2);
-                    if (spectral)
-                        b200pt_s60::launch_shade(s60(r->d_dev), m, full_shade, b, wk + 1 + m, r->grid_shade_s60, st);
-                    else
-                        launch_shade(r->d_dev, m, full_shade, b, wk + 1 + m, r->grid_shade, st);
+                    LAUNCH_SPEC(launch_shade, dev, m, full_shade, b, wk + W_SHADE0 + m, spectral ? r->grid_shade_s60 : r->grid_shade, st);
                 }
             if (b < maxDepth && medium) {
                 // the medium pass of bounce b+1 writes the same per-slot direct-lighting records: finish bounce b's first
                 trace_direct(b);
                 {
                     LaunchTimer lt(r, st, 2);
-                    if (spectral)
-                        b200pt_s60::launch_resolve(s60(r->d_dev), b, wk + 7, r->grid_shade, st);
-                    else
-                        launch_resolve(r->d_dev, b, wk + 7, r->grid_shade, st);
+                    LAUNCH_SPEC(launch_resolve, dev, b, wk + W_RESOLVE, r->grid_shade, st);
                 }
                 trace_path(b + 1);
             } else if (b < maxDepth) {  // no direct lighting is estimated at the last vertex (path.cpp:104)
@@ -1662,22 +1654,15 @@ int b200pt_render_tiles(b200pt_render *r, const int32_t *tiles, int64_t n_tiles)
                 trace_path(b + 1);
                 if (overlap) CUDA_TRY(cudaStreamWaitEvent(st, ctx->ev_join, 0));
                 LaunchTimer lt(r, st, 2);
-                if (spectral)
-                    b200pt_s60::launch_resolve(s60(r->d_dev), b, wk + 7, r->grid_shade, st);
-                else
-                    launch_resolve(r->d_dev, b, wk + 7, r->grid_shade, st);
+                LAUNCH_SPEC(launch_resolve, dev, b, wk + W_RESOLVE, r->grid_shade, st);
             }
         }
         {
             LaunchTimer lt(r, st, 2);
-            if (H.filter_general && spectral)
-                b200pt_s60::launch_film_general(s60(r->d_dev), s60(H), (uint32_t)first, nb, st);
-            else if (H.filter_general)
-                launch_film_general(r->d_dev, H, (uint32_t)first, nb, st);
-            else if (spectral)
-                b200pt_s60::launch_film(s60(r->d_dev), (uint32_t)first, nb, st);
+            if (H.filter_general)
+                LAUNCH_SPEC(launch_film_general, dev, host, (uint32_t)first, nb, st);
             else
-                launch_film(r->d_dev, (uint32_t)first, nb, st);
+                LAUNCH_SPEC(launch_film, dev, (uint32_t)first, nb, st);
         }
         launch_accumulate_stats(r->d_dev, 0, st);
         r->launches++;
@@ -1685,6 +1670,7 @@ int b200pt_render_tiles(b200pt_render *r, const int32_t *tiles, int64_t n_tiles)
     }
     return B200PT_OK;
 }
+#undef LAUNCH_SPEC
 
 int b200pt_film_device_buffer(b200pt_render *r, uint64_t *dev_ptr, uint64_t *n_floats) {
     if (!r) return b200pt_fail(B200PT_ERR_INVALID, "render is NULL");

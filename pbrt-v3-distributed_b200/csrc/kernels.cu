@@ -139,14 +139,14 @@ template <bool VTX>
 __device__ __forceinline__ void load_shading(const DevScene &sc, uint32_t ti, uint32_t mflags, TriShading *t) {
     default_shading(t);
     if (!VTX) return;
-    if (mflags & 0x40000u) {
+    if (mflags & B200PT_TRI_HAS_NORMALS) {
         const F4 *np = sc.tri_n + (size_t)ti * 3;
         t->has_n = 1;
         t->n0 = v3(ld_f4(np));
         t->n1 = v3(ld_f4(np + 1));
         t->n2 = v3(ld_f4(np + 2));
     }
-    if (mflags & 0x80000u) {
+    if (mflags & B200PT_TRI_HAS_UVS) {
         const F4 a = ld_f4(sc.tri_uv + (size_t)ti * 2), b = ld_f4(sc.tri_uv + (size_t)ti * 2 + 1);
         t->uv[0] = a.x;
         t->uv[1] = a.y;
@@ -154,6 +154,19 @@ __device__ __forceinline__ void load_shading(const DevScene &sc, uint32_t ti, ui
         t->uv[3] = a.w;
         t->uv[4] = b.x;
         t->uv[5] = b.y;
+    }
+}
+
+// ---- classification of closest hits, shared by the traversal kernels and the medium passes
+// BSDF family (the queue, the k_shade instance) of a hit with material word `mflags`
+__device__ __forceinline__ int hit_family(const b200pt_material *materials, uint32_t mflags) { return materials[mflags & 0xffffu].type; }
+// Appends `slot` to the queue of BSDF family `family` (-1: to none).  Every lane of the warp must call it (converged).
+__device__ __forceinline__ void append_family(uint32_t *const *q_mat, uint32_t *qcount_mat, int family, uint32_t slot) {
+#pragma unroll
+    for (int m = 0; m < 4; ++m) {
+        const bool mine = family == m;
+        const uint32_t pos = warp_append(&qcount_mat[m], mine);
+        if (mine) q_mat[m][pos] = slot;
     }
 }
 
@@ -278,11 +291,8 @@ void k_trace(const TraceArgs a) {
             r.b1 = hit.b1;
             a.full_out[slot] = r;
         }
-        if (CLASSIFY && best != B200PT_MISS) {
-            const uint32_t mf = __float_as_uint(ld_f4(a.tris + (size_t)best * 3 + 1).w);
-            const int family = a.materials[mf & 0xffffu].type;
-            a.q_mat[family][warp_append(&a.qcount_mat[family], true)] = slot;
-        }
+        if (CLASSIFY && best != B200PT_MISS)
+            append_family(a.q_mat, a.qcount_mat, hit_family(a.materials, __float_as_uint(ld_f4(a.tris + (size_t)best * 3 + 1).w)), slot);
     }
     if (COUNT) {
         atomicAdd(&a.stats[ANY_HIT ? 5 : 3], (unsigned long long)ctr.nodes);
@@ -384,21 +394,12 @@ __global__ void __launch_bounds__(128, B200PT_TRACE_CTAS) k_trace(const TraceArg
                         r.b1 = my_ray[11 * 128];
                         a.full_out[slot] = r;
                     }
-                    if (CLASSIFY && best != B200PT_MISS) {
-                        const uint32_t mf = __float_as_uint(ld_f4(a.tris + (size_t)best * 3 + 1).w);
-                        family = a.materials[mf & 0xffffu].type;
-                    }
+                    if (CLASSIFY && best != B200PT_MISS)
+                        family = hit_family(a.materials, __float_as_uint(ld_f4(a.tris + (size_t)best * 3 + 1).w));
                 }
                 if ((T.sp & B200PT_SP_OVERFLOW) && a.stats) atomicAdd(&a.stats[7], 1ull);
             }
-            if (CLASSIFY) {
-#pragma unroll
-                for (int m = 0; m < 4; ++m) {
-                    const bool mine = family == m;
-                    const uint32_t pos = warp_append(&a.qcount_mat[m], mine);
-                    if (mine) a.q_mat[m][pos] = slot;
-                }
-            }
+            if (CLASSIFY) append_family(a.q_mat, a.qcount_mat, family, slot);
             fin = false;
         }
         // ---- converged: idle lanes fetch new rays
@@ -573,21 +574,12 @@ __global__ void __launch_bounds__(128, 6) k_trace2(const TraceArgs a) {
                         r.b1 = my_ray[11 * 128];
                         a.full_out[slot] = r;
                     }
-                    if (CLASSIFY && best != B200PT_MISS) {
-                        const uint32_t mf = __float_as_uint(ld_f4(a.tris + (size_t)best * 3 + 1).w);
-                        family = a.materials[mf & 0xffffu].type;
-                    }
+                    if (CLASSIFY && best != B200PT_MISS)
+                        family = hit_family(a.materials, __float_as_uint(ld_f4(a.tris + (size_t)best * 3 + 1).w));
                 }
                 if ((T.sp & B200PT_SP_OVERFLOW) && a.stats) atomicAdd(&a.stats[7], 1ull);
             }
-            if (CLASSIFY) {
-#pragma unroll
-                for (int m = 0; m < 4; ++m) {
-                    const bool mine = family == m;
-                    const uint32_t pos = warp_append(&a.qcount_mat[m], mine);
-                    if (mine) a.q_mat[m][pos] = slot;
-                }
-            }
+            if (CLASSIFY) append_family(a.q_mat, a.qcount_mat, family, slot);
             fin = false;
         }
         // ---- converged: idle lanes fetch new rays
@@ -953,18 +945,11 @@ __global__ void __launch_bounds__(128) k_spheres(const TraceArgs a) {
                     if (CLASSIFY && best != B200PT_MISS) {
                         const uint32_t mf = is_sphere_hit(best) ? a.spheres[best & SPHERE_HIT_MASK].mat_flags
                                                                 : __float_as_uint(ld_f4(a.tris + (size_t)best * 3 + 1).w);
-                        family = a.materials[mf & 0xffffu].type;
+                        family = hit_family(a.materials, mf);
                     }
                 }
             }
-            if (CLASSIFY) {
-#pragma unroll
-                for (int m = 0; m < 4; ++m) {
-                    const bool mine = family == m;
-                    const uint32_t pos = warp_append(&a.qcount_mat[m], mine);
-                    if (mine) a.q_mat[m][pos] = slot;
-                }
-            }
+            if (CLASSIFY) append_family(a.q_mat, a.qcount_mat, family, slot);
             fin = false;
         }
         // ---- converged: idle lanes fetch new rays, test the spheres, set up the walk over the instances
@@ -1016,7 +1001,7 @@ __global__ void __launch_bounds__(128) k_spheres(const TraceArgs a) {
                             const F4 *tp = a.tris + (size_t)best * 3;
                             const F4 t0 = ld_f4(tp), t1 = ld_f4(tp + 1), t2 = ld_f4(tp + 2);
                             V3 o2 = ro, d2 = rd;
-                            if ((__float_as_uint(t1.w) & 0x100000u) && a.hit_inst_out) {
+                            if ((__float_as_uint(t1.w) & B200PT_TRI_INSTANCED) && a.hit_inst_out) {
                                 // a triangle of an instanced object (found by the two-level kernel): the same ray parameter in
                                 // the object's space (primitive.cpp:91)
                                 float tm2;
@@ -1176,7 +1161,7 @@ __device__ void estimate_direct(const RenderDev *R, const Isect &is, const Bsdf 
     }
     const V3 p0 = v3(t0), p1 = v3(t1), p2 = v3(t2);
     const uint32_t lflags = __float_as_uint(t1.w);
-    const bool lflip = (lflags & 0x10000u) != 0, ldegenerate = (lflags & 0x20000u) != 0;
+    const bool lflip = (lflags & B200PT_TRI_FLIP) != 0, ldegenerate = (lflags & B200PT_TRI_DEGENERATE) != 0;
     TriShading lsh;
     load_shading<VTX>(R->scene, light.tri, lflags, &lsh);
     const Spec lemit = light_emit(R, lightNum, light);
@@ -1311,6 +1296,188 @@ __device__ __forceinline__ void store_direct_general(const RenderDev *R, uint32_
 #endif
 }
 
+// ------------------------------------------------------------------ path-vertex steps
+// One copy of each step shared by the kernels that process a path vertex per lane: k_shade of either spectrum build,
+// k_medium and k_medium_general.
+
+// The path ray of a slot and the fields of its meta word (PathRec::o / PathRec::d)
+struct PathVertex {
+    V3 ro, rd;
+    float etaScale;
+    uint32_t meta;
+    int bounces;
+    bool specularBounce;
+};
+__device__ __forceinline__ PathVertex load_vertex(const PathRec &P) {
+    const float4 o4 = P.o, d4 = P.d;
+    PathVertex v;
+    v.ro = v3(o4);
+    v.rd = v3(d4);
+    v.etaScale = o4.w;
+    v.meta = __float_as_uint(d4.w);
+    v.bounces = (int)((v.meta >> 16) & 0xffu);
+    v.specularBounce = ((v.meta >> 24) & PF_SPECULAR) != 0;
+    return v;
+}
+// the sampler of a path, continued at the dimension its meta word holds
+__device__ __forceinline__ SobolStream sobol_stream(uint64_t index, uint32_t meta) {
+    SobolStream st;
+    st.index = index;
+    st.dim = (int)(meta & 0xffffu);
+    st.px = st.py = 0;  // only dimensions 0/1 depend on the pixel
+    return st;
+}
+__device__ __forceinline__ uint32_t pack_meta(int dim, int bounces, bool specular) {
+    return ((uint32_t)dim & 0xffffu) | ((uint32_t)bounces << 16) | ((specular ? (uint32_t)PF_SPECULAR : 0u) << 24);
+}
+// the meta word of a path that stays on its bounce (bounces and flags kept) after it spent sampler dimensions
+__device__ __forceinline__ uint32_t meta_with_dim(uint32_t meta, int dim) { return (meta & 0xffff0000u) | ((uint32_t)dim & 0xffffu); }
+
+// Re-derives the accepted closest hit P.hit of the path ray as a surface interaction: Shape::Intersect's values (t, b0,
+// b1, b2, or the sphere's root) do not depend on tMax.  Fills the hit's material word and light id too.
+template <bool VTX>
+__device__ __forceinline__ bool accepted_hit(const RenderDev *R, const PathRec &P, const V3 &ro, const V3 &rd, Isect *is, uint32_t *mflags,
+                                             int *lightId) {
+    const uint32_t ti = P.hit;
+    bool found;
+    if (VTX && is_sphere_hit(ti)) {
+        const DevSphere *sp = R->scene.spheres + (ti & SPHERE_HIT_MASK);
+        float th;
+        found = sphere_intersect(*sp, ro, rd, pt_inf(), &th, is);
+        *mflags = sp->mat_flags;
+        *lightId = sp->light_id;
+    } else {
+        const F4 *tp = R->scene.tris + (size_t)ti * 3;
+        const F4 t0 = ld_f4(tp), t1 = ld_f4(tp + 1), t2 = ld_f4(tp + 2);
+        const V3 p0 = v3(t0), p1 = v3(t1), p2 = v3(t2);
+        *mflags = __float_as_uint(t1.w);
+        *lightId = (int)__float_as_uint(t2.w);
+        TriHit h;
+        if (VTX && (*mflags & B200PT_TRI_INSTANCED)) {
+            // a triangle of an instanced object: intersect in the object's space, bring the hit back
+            const DevInstance *in = R->scene.instances + P.hit_inst;
+            V3 o2, d2;
+            float tm2;
+            instance_ray(*in, ro, rd, pt_inf(), &o2, &d2, &tm2);
+            found = triangle_test(p0, p1, p2, o2, make_shear(d2), pt_inf(), &h);
+            if (found) {
+                TriShading tsh;
+                load_shading<VTX>(R->scene, ti, *mflags, &tsh);
+                fill_isect(p0, p1, p2, (*mflags & B200PT_TRI_FLIP) != 0, tsh, h, d2, is);
+                instance_isect_to_world(*in, is);
+            }
+        } else {
+            found = triangle_test(p0, p1, p2, ro, make_shear(rd), pt_inf(), &h);
+            if (found) {
+                TriShading tsh;
+                load_shading<VTX>(R->scene, ti, *mflags, &tsh);
+                fill_isect(p0, p1, p2, (*mflags & B200PT_TRI_FLIP) != 0, tsh, h, rd, is);
+            }
+        }
+    }
+    return found;
+}
+// Distance of the closest hit `ti` = P.hit along (ro, rd) -- ray.tMax after Scene::Intersect, infinity for a miss -- and
+// the hit's material word.  (k_medium_general never meets an instanced triangle: render_create refuses bounded media in
+// scenes with object instances.)
+__device__ __forceinline__ float hit_distance(const RenderDev *R, const PathRec &P, uint32_t ti, const V3 &ro, const V3 &rd,
+                                              uint32_t *mflags) {
+    float tHit = pt_inf();
+    *mflags = 0;
+    if (ti == B200PT_MISS) return tHit;
+    if (is_sphere_hit(ti)) {
+        const DevSphere *sp = R->scene.spheres + (ti & SPHERE_HIT_MASK);
+        float th;
+        if (sphere_intersect(*sp, ro, rd, pt_inf(), &th, nullptr)) tHit = th;
+        *mflags = sp->mat_flags;
+    } else {
+        const F4 *tp = R->scene.tris + (size_t)ti * 3;
+        const F4 t0 = ld_f4(tp), t1 = ld_f4(tp + 1), t2 = ld_f4(tp + 2);
+        *mflags = __float_as_uint(t1.w);
+        V3 o2 = ro, d2 = rd;
+        if (*mflags & B200PT_TRI_INSTANCED) {  // a triangle of an instanced object: same ray parameter in the object's space
+            float tm2;
+            instance_ray(R->scene.instances[P.hit_inst], ro, rd, pt_inf(), &o2, &d2, &tm2);
+        }
+        TriHit h;
+        if (triangle_test(v3(t0), v3(t1), v3(t2), o2, make_shear(d2), pt_inf(), &h)) tHit = h.t;
+    }
+    return tHit;
+}
+// lightDistribution->Lookup(p) (path.cpp:115: the uniform / power table, or the table of p's voxel) and
+// SampleDiscrete(u) on it (UniformSampleOneLight, integrator.cpp:85-106)
+__device__ __forceinline__ int pick_light(const RenderDev *R, const V3 &p, float u, float *pickPdf) {
+    const float *cdf = R->light_cdf, *func = R->light_func;
+    float funcInt = R->light_func_int;
+    if (R->grid.enabled) {
+        const int vox = spatial_voxel(R->grid, p);
+        cdf = R->sp_cdf + (size_t)vox * (R->n_lights + 1);
+        func = R->sp_func + (size_t)vox * R->n_lights;
+        funcInt = R->sp_func_int[vox];
+    }
+    return sample_discrete(cdf, func, funcInt, R->n_lights, u, pickPdf);
+}
+// MediumInteraction(ray(t), -ray.d, ...): no normal, no error bounds
+__device__ __forceinline__ Isect medium_interaction(const V3 &ro, const V3 &rd, float t) {
+    Isect mi;
+    mi.p = ro + rd * t;
+    mi.wo = -rd;
+    mi.n = mi.ns = mk(0.f, 0.f, 0.f);
+    mi.pError = mk(0.f, 0.f, 0.f);
+    return mi;
+}
+// HomogeneousMedium::Sample (homogeneous.cpp:49-76) on an eager spectrum: the channel and the free-flight distance against
+// the distance tHit of the hit, beta *= Tr [* sigma_s] / pdf.  Returns t; *sampledMedium: the path scatters at ray(t).
+__device__ __forceinline__ float sample_medium_rgb(const Spec &sigmaT, const Spec &sigmaS, const V3 &rd, float tHit, float uChannel,
+                                                   float uDist, Spec *beta, bool *sampledMedium) {
+    const int channel = pt_mini((int)(uChannel * B200PT_NSPEC), B200PT_NSPEC - 1);
+    const float dist = -pt_logf(1 - uDist) / sigmaT.c[channel];
+    const float rdLen = len(rd);
+    const float t = pt_min(dist / rdLen, tHit);
+    *sampledMedium = t < tHit;
+    Spec Tr;
+    PT_UNROLL SPEC_FOR Tr.c[i_] = pt_expf((-sigmaT.c[i_]) * pt_min(t, PT_MAX_FLOAT) * rdLen);
+    const Spec density = *sampledMedium ? (sigmaT * Tr) : Tr;
+    float pdf = 0.f;
+    SPEC_FOR pdf += density.c[i_];
+    pdf *= 1 / (float)B200PT_NSPEC;
+    if (pdf == 0) pdf = 1;
+    *beta = *beta * (*sampledMedium ? (Tr * sigmaS / pdf) : (Tr / pdf));
+    return t;
+}
+// Russian roulette (path.cpp:176-184) of a path whose rrMax = max(beta * etaScale) is below the threshold, with the
+// sample u the caller drew for it: false ends the path, otherwise beta /= 1 - q.
+__device__ __forceinline__ bool russian_roulette(float rrMax, float u, Spec *beta) {
+    const float q = pt_max(.05f, 1 - rrMax);
+    if (u < q) return false;
+    *beta = *beta / (1 - q);
+    return true;
+}
+// ... with beta streamed through the slot's 60 bins
+__device__ __forceinline__ bool russian_roulette(float rrMax, float u, float4 *sBeta) {
+    const float q = pt_max(.05f, 1 - rrMax);
+    if (u < q) return false;
+    const float dq = 1 - q;
+#pragma unroll 5
+    for (int q4 = 0; q4 < B200PT_NSPEC / 4; ++q4) {
+        const float4 v = sBeta[q4];
+        sBeta[q4] = make_float4(v.x / dq, v.y / dq, v.z / dq, v.w / dq);
+    }
+    return true;
+}
+
+// What a vertex leaves behind: its pending shadow and MIS rays (counters in the bounce's block qc) and the path itself
+// if it goes on.  Every lane of the warp must call it (converged).
+__device__ __forceinline__ void append_vertex_out(const RenderDev *R, uint32_t *qc, uint32_t *qc_next, uint32_t *q_next, uint32_t pend,
+                                                  bool cont, uint32_t slot) {
+    const uint32_t ps = warp_append(&qc[Q_SHADOW], (pend & PEND_LIGHT) != 0);
+    if (pend & PEND_LIGHT) R->q_shadow[ps] = slot;
+    const uint32_t pm = warp_append(&qc[Q_MIS], (pend & PEND_BSDF) != 0);
+    if (pend & PEND_BSDF) R->q_mis[pm] = slot;
+    const uint32_t pn = warp_append(qc_next, cont);
+    if (cont) q_next[pn] = slot;
+}
+
 #if B200PT_NSPEC == 3
 // resident CTAs per SM the shading kernels are compiled for (4 -> 128 registers; A/B builds: 5 -> 96, 6 -> 80)
 #ifndef B200PT_SHADE_MINCTAS
@@ -1318,131 +1485,46 @@ __device__ __forceinline__ void store_direct_general(const RenderDev *R, uint32_
 #endif
 template <int MAT, bool VTX>
 __global__ void __launch_bounds__(128, B200PT_SHADE_MINCTAS) k_shade(const RenderDev *R, int bounce, uint32_t *work) {
-    const uint32_t n = R->qcount[bounce * Q_PER_BOUNCE + Q_MAT0 + MAT];
+    uint32_t *qc = &R->qcount[bounce * Q_PER_BOUNCE];
+    const uint32_t n = qc[Q_MAT0 + MAT];
     const uint32_t *queue = R->q_mat[MAT];
     uint32_t *qc_next = &R->qcount[(bounce + 1) * Q_PER_BOUNCE + Q_PATH];
-    uint32_t *qc_shadow = &R->qcount[bounce * Q_PER_BOUNCE + Q_SHADOW];
-    uint32_t *qc_mis = &R->qcount[bounce * Q_PER_BOUNCE + Q_MIS];
     uint32_t *q_next = R->q_path[(bounce + 1) & 1];
     uint32_t i;
-#if defined(B200PT_SHADE_PREFETCH) && !defined(B200PT_HOST_EMU)
-    // A/B build: the next work item is fetched one iteration ahead and its state (slot record, hit triangle) is pulled
-    // towards the SM while the current vertex is shaded -- the chain queue -> slot -> hit -> triangle is four dependent
-    // DRAM accesses otherwise
-    uint32_t i_next = 0, slot_next = 0, hit_next = B200PT_MISS;
-    bool have = warp_fetch(work, n, &i_next);
-    if (have && i_next < n) {
-        slot_next = queue[i_next];
-        hit_next = R->path[slot_next].hit;
-    }
-    while (have) {
-        i = i_next;
-        const uint32_t slot_cur = slot_next;
-        have = warp_fetch(work, n, &i_next);
-        slot_next = 0;
-        hit_next = B200PT_MISS;
-        if (have && i_next < n) {
-            slot_next = queue[i_next];
-            asm volatile("prefetch.global.L2 [%0];" ::"l"(&R->path[slot_next].o));
-            asm volatile("prefetch.global.L2 [%0];" ::"l"(&R->path[slot_next].beta));
-            asm volatile("prefetch.global.L2 [%0];" ::"l"(&R->path[slot_next].sobol));
-            hit_next = R->path[slot_next].hit;
-        }
-#else
     while (warp_fetch(work, n, &i)) {
-#endif
         const bool active = i < n;
         bool cont = false;
         uint32_t pend = 0, slot = 0;
         if (active) {
-#if defined(B200PT_SHADE_PREFETCH) && !defined(B200PT_HOST_EMU)
-            slot = slot_cur;
-#else
             slot = queue[i];
-#endif
             PathRec &P = R->path[slot];
-            const float4 o4 = P.o, d4 = P.d;
+            PathVertex v = load_vertex(P);
             float betaW, LW;
             Spec beta = ld_spec(P.beta, R->s_beta, slot, &betaW);
             Spec L = ld_spec(P.L, R->s_L, slot, &LW);
-            const V3 ro = v3(o4), rd = v3(d4);
-            float etaScale = o4.w;
-            const uint32_t meta = __float_as_uint(d4.w);
-            const int bounces = (int)((meta >> 16) & 0xffu);
-            const bool specularBounce = ((meta >> 24) & PF_SPECULAR) != 0;
-            const uint32_t ti = P.hit;
             Isect is;
             uint32_t mflags;
             int lightId;
-            bool found;
-            if (VTX && is_sphere_hit(ti)) {
-                // the accepted root does not depend on tMax either (t0 unless its interval reaches 0, then t1)
-                const DevSphere *sp = R->scene.spheres + (ti & SPHERE_HIT_MASK);
-                float th;
-                found = sphere_intersect(*sp, ro, rd, pt_inf(), &th, &is);
-                mflags = sp->mat_flags;
-                lightId = sp->light_id;
-            } else {
-                const F4 *tp = R->scene.tris + (size_t)ti * 3;
-                const F4 t0 = ld_f4(tp), t1 = ld_f4(tp + 1), t2 = ld_f4(tp + 2);
-                const V3 p0 = v3(t0), p1 = v3(t1), p2 = v3(t2);
-                mflags = __float_as_uint(t1.w);
-                lightId = (int)__float_as_uint(t2.w);
-                // re-derive (t, b0, b1, b2) of the accepted hit: Triangle::Intersect's values do not depend on tMax
-                TriHit h;
-                if (VTX && (mflags & 0x100000u)) {
-                    // a triangle of an instanced object: intersect in the object's space, bring the hit back
-                    const DevInstance *in = R->scene.instances + P.hit_inst;
-                    V3 o2, d2;
-                    float tm2;
-                    instance_ray(*in, ro, rd, pt_inf(), &o2, &d2, &tm2);
-                    found = triangle_test(p0, p1, p2, o2, make_shear(d2), pt_inf(), &h);
-                    if (found) {
-                        TriShading tsh;
-                        load_shading<VTX>(R->scene, ti, mflags, &tsh);
-                        fill_isect(p0, p1, p2, (mflags & 0x10000u) != 0, tsh, h, d2, &is);
-                        instance_isect_to_world(*in, &is);
-                    }
-                } else {
-                    found = triangle_test(p0, p1, p2, ro, make_shear(rd), pt_inf(), &h);
-                    if (found) {
-                        TriShading tsh;
-                        load_shading<VTX>(R->scene, ti, mflags, &tsh);
-                        fill_isect(p0, p1, p2, (mflags & 0x10000u) != 0, tsh, h, rd, &is);
-                    }
-                }
-            }
-            if (found) {
+            if (accepted_hit<VTX>(R, P, v.ro, v.rd, &is, &mflags, &lightId)) {
                 // path.cpp:91-101: emitted light at the first vertex or after a specular bounce
-                if (bounces == 0 || specularBounce) {
+                if (v.bounces == 0 || v.specularBounce) {
                     if (lightId >= 0) {
                         const DevLight lt = R->lights[lightId];
-                        const Spec Le = (lt.two_sided || dot(is.n, -rd) > 0) ? light_emit(R, lightId, lt) : rgb1(0.f);
+                        const Spec Le = (lt.two_sided || dot(is.n, -v.rd) > 0) ? light_emit(R, lightId, lt) : rgb1(0.f);
                         L = L + beta * Le;
                     }
                 }
-                if (bounces < R->max_depth) {  // path.cpp:104
+                if (v.bounces < R->max_depth) {  // path.cpp:104
                     Bsdf bsdf;
                     const uint32_t mi = mflags & 0xffffu;
                     make_bsdf<MAT>(R->scene.materials[mi], R->scene.material_spectra + (size_t)mi * (5 * B200PT_NSPEC), is, &bsdf);
-                    SobolStream st;
-                    st.index = P.sobol;
-                    st.dim = (int)(meta & 0xffffu);
-                    st.px = st.py = 0;  // only dimensions 0/1 depend on the pixel
+                    SobolStream st = sobol_stream(P.sobol, v.meta);
                     const SamplerParams &sp = R->sampler;
                     // path.cpp:119-128 -> UniformSampleOneLight (integrator.cpp:85-106)
                     // (VolPathIntegrator samples a light at every surface vertex, volpath.cpp:124-128)
                     if (((VTX && R->volpath) || bsdf_num_components(bsdf, BSDF_ALL & ~BSDF_SPECULAR) > 0) && R->n_lights > 0) {
                         float pickPdf;
-                        const float *cdf = R->light_cdf, *func = R->light_func;
-                        float funcInt = R->light_func_int;
-                        if (R->grid.enabled) {  // lightDistribution->Lookup(isect.p), path.cpp:115
-                            const int vox = spatial_voxel(R->grid, is.p);
-                            cdf = R->sp_cdf + (size_t)vox * (R->n_lights + 1);
-                            func = R->sp_func + (size_t)vox * R->n_lights;
-                            funcInt = R->sp_func_int[vox];
-                        }
-                        const int lightNum = sample_discrete(cdf, func, funcInt, R->n_lights, get1d(sp, st), &pickPdf);
+                        const int lightNum = pick_light(R, is.p, get1d(sp, st), &pickPdf);
                         if (pickPdf != 0) {
                             float uLight[2], uScattering[2];
                             get2d(sp, st, uLight);
@@ -1469,7 +1551,7 @@ __global__ void __launch_bounds__(128, B200PT_SHADE_MINCTAS) k_shade(const Rende
                         }
                     }
                     // path.cpp:131-150: sample the BSDF for the next direction
-                    const V3 wo = -rd;
+                    const V3 wo = -v.rd;
                     V3 wi = mk(0.f, 0.f, 0.f);
                     float pdf = 0.f;
                     int flags = 0;
@@ -1481,24 +1563,15 @@ __global__ void __launch_bounds__(128, B200PT_SHADE_MINCTAS) k_shade(const Rende
                         const bool spec = (flags & BSDF_SPECULAR) != 0;
                         if ((flags & BSDF_SPECULAR) && (flags & BSDF_TRANSMISSION)) {
                             const float eta = bsdf.eta;
-                            etaScale *= (dot(wo, is.n) > 0) ? (eta * eta) : 1 / (eta * eta);
+                            v.etaScale *= (dot(wo, is.n) > 0) ? (eta * eta) : 1 / (eta * eta);
                         }
                         const V3 no = offset_ray_origin(is.p, is.pError, is.n, wi);  // isect.SpawnRay(wi)
                         cont = true;
-                        // path.cpp:176-184: Russian roulette
-                        const Spec rrBeta = beta * etaScale;
-                        if (max_comp(rrBeta) < R->rr_threshold && bounces > 3) {
-                            const float q = pt_max(.05f, 1 - max_comp(rrBeta));
-                            if (get1d(sp, st) < q)
-                                cont = false;
-                            else
-                                beta = beta / (1 - q);
-                        }
+                        const float rrMax = max_comp(beta * v.etaScale);
+                        if (rrMax < R->rr_threshold && v.bounces > 3) cont = russian_roulette(rrMax, get1d(sp, st), &beta);
                         if (cont) {
-                            const uint32_t nmeta = ((uint32_t)st.dim & 0xffffu) | ((uint32_t)(bounces + 1) << 16) |
-                                                   ((spec ? (uint32_t)PF_SPECULAR : 0u) << 24);
-                            P.o = f4(no, etaScale);
-                            P.d = f4(wi, __uint_as_float(nmeta));
+                            P.o = f4(no, v.etaScale);
+                            P.d = f4(wi, __uint_as_float(pack_meta(st.dim, v.bounces + 1, spec)));
                             betaW = 0.f;
                         }
                     }
@@ -1508,19 +1581,7 @@ __global__ void __launch_bounds__(128, B200PT_SHADE_MINCTAS) k_shade(const Rende
                 st_spec(P.L, R->s_L, slot, L, LW);
             }
         }
-        const uint32_t ps = warp_append(qc_shadow, (pend & PEND_LIGHT) != 0);
-        if (pend & PEND_LIGHT) R->q_shadow[ps] = slot;
-        const uint32_t pm = warp_append(qc_mis, (pend & PEND_BSDF) != 0);
-        if (pend & PEND_BSDF) R->q_mis[pm] = slot;
-        const uint32_t pn = warp_append(qc_next, cont);
-        if (cont) q_next[pn] = slot;
-#if defined(B200PT_SHADE_PREFETCH) && !defined(B200PT_HOST_EMU)
-        if (hit_next != B200PT_MISS && !is_sphere_hit(hit_next)) {
-            const F4 *tp = R->scene.tris + (size_t)hit_next * 3;
-            asm volatile("prefetch.global.L2 [%0];" ::"l"(tp));
-            asm volatile("prefetch.global.L2 [%0];" ::"l"(tp + 2));
-        }
-#endif
+        append_vertex_out(R, qc, qc_next, q_next, pend, cont, slot);
     }
 }
 
@@ -1649,7 +1710,7 @@ __device__ void estimate_direct_lazy(const RenderDev *R, uint32_t slot, const Is
     }
     const V3 p0 = v3(t0), p1 = v3(t1), p2 = v3(t2);
     const uint32_t lflags = __float_as_uint(t1.w);
-    const bool lflip = (lflags & 0x10000u) != 0, ldegenerate = (lflags & 0x20000u) != 0;
+    const bool lflip = (lflags & B200PT_TRI_FLIP) != 0, ldegenerate = (lflags & B200PT_TRI_DEGENERATE) != 0;
     TriShading lsh;
     load_shading<true>(R->scene, light.tri, lflags, &lsh);
     const int flagsNS = BSDF_ALL & ~BSDF_SPECULAR;
@@ -1790,11 +1851,10 @@ __device__ void estimate_direct_lazy(const RenderDev *R, uint32_t slot, const Is
 #endif
 template <int MAT, bool VTX>
 __global__ void __launch_bounds__(128, B200PT_S60_SHADE_MINCTAS) k_shade(const RenderDev *R, int bounce, uint32_t *work) {
-    const uint32_t n = R->qcount[bounce * Q_PER_BOUNCE + Q_MAT0 + MAT];
+    uint32_t *qc = &R->qcount[bounce * Q_PER_BOUNCE];
+    const uint32_t n = qc[Q_MAT0 + MAT];
     const uint32_t *queue = R->q_mat[MAT];
     uint32_t *qc_next = &R->qcount[(bounce + 1) * Q_PER_BOUNCE + Q_PATH];
-    uint32_t *qc_shadow = &R->qcount[bounce * Q_PER_BOUNCE + Q_SHADOW];
-    uint32_t *qc_mis = &R->qcount[bounce * Q_PER_BOUNCE + Q_MIS];
     uint32_t *q_next = R->q_path[(bounce + 1) & 1];
     uint32_t i;
     while (warp_fetch(work, n, &i)) {
@@ -1803,58 +1863,18 @@ __global__ void __launch_bounds__(128, B200PT_S60_SHADE_MINCTAS) k_shade(const R
         uint32_t pend = 0, slot = 0;
         if (active) {
             slot = queue[i];
-            const float4 o4 = R->path[slot].o, d4 = R->path[slot].d;
+            PathRec &P = R->path[slot];
+            PathVertex v = load_vertex(P);
             float4 *sBeta = reinterpret_cast<float4 *>(R->s_beta + (size_t)slot * B200PT_NSPEC);
             float4 *sL = reinterpret_cast<float4 *>(R->s_L + (size_t)slot * B200PT_NSPEC);
-            const V3 ro = v3(o4), rd = v3(d4);
-            float etaScale = o4.w;
-            const uint32_t meta = __float_as_uint(d4.w);
-            const int bounces = (int)((meta >> 16) & 0xffu);
-            const bool specularBounce = ((meta >> 24) & PF_SPECULAR) != 0;
-            const uint32_t ti = R->path[slot].hit;
             Isect is;
             uint32_t mflags;
             int lightId;
-            bool found;
-            if (is_sphere_hit(ti)) {
-                const DevSphere *sp = R->scene.spheres + (ti & SPHERE_HIT_MASK);
-                float th;
-                found = sphere_intersect(*sp, ro, rd, pt_inf(), &th, &is);
-                mflags = sp->mat_flags;
-                lightId = sp->light_id;
-            } else {
-                const F4 *tp = R->scene.tris + (size_t)ti * 3;
-                const F4 t0 = ld_f4(tp), t1 = ld_f4(tp + 1), t2 = ld_f4(tp + 2);
-                const V3 p0 = v3(t0), p1 = v3(t1), p2 = v3(t2);
-                mflags = __float_as_uint(t1.w);
-                lightId = (int)__float_as_uint(t2.w);
-                TriHit h;
-                if (mflags & 0x100000u) {
-                    const DevInstance *in = R->scene.instances + R->path[slot].hit_inst;
-                    V3 o2, d2;
-                    float tm2;
-                    instance_ray(*in, ro, rd, pt_inf(), &o2, &d2, &tm2);
-                    found = triangle_test(p0, p1, p2, o2, make_shear(d2), pt_inf(), &h);
-                    if (found) {
-                        TriShading tsh;
-                        load_shading<true>(R->scene, ti, mflags, &tsh);
-                        fill_isect(p0, p1, p2, (mflags & 0x10000u) != 0, tsh, h, d2, &is);
-                        instance_isect_to_world(*in, &is);
-                    }
-                } else {
-                    found = triangle_test(p0, p1, p2, ro, make_shear(rd), pt_inf(), &h);
-                    if (found) {
-                        TriShading tsh;
-                        load_shading<true>(R->scene, ti, mflags, &tsh);
-                        fill_isect(p0, p1, p2, (mflags & 0x10000u) != 0, tsh, h, rd, &is);
-                    }
-                }
-            }
-            if (found) {
+            if (accepted_hit<true>(R, P, v.ro, v.rd, &is, &mflags, &lightId)) {
                 // path.cpp:91-101: L += beta * Le at the first vertex or after a specular bounce
-                if ((bounces == 0 || specularBounce) && lightId >= 0) {
+                if ((v.bounces == 0 || v.specularBounce) && lightId >= 0) {
                     const DevLight &lt = R->lights[lightId];
-                    if (lt.two_sided || dot(is.n, -rd) > 0) {
+                    if (lt.two_sided || dot(is.n, -v.rd) > 0) {
                         const float *le = R->light_spectra + (size_t)lightId * B200PT_NSPEC;
 #pragma unroll 3
                         for (int q = 0; q < B200PT_NSPEC / 4; ++q) {
@@ -1866,26 +1886,15 @@ __global__ void __launch_bounds__(128, B200PT_S60_SHADE_MINCTAS) k_shade(const R
                         // L + beta * 0: only a -0 would change, and L never holds one (it starts at +0 and only sums)
                     }
                 }
-                if (bounces < R->max_depth) {
+                if (v.bounces < R->max_depth) {
                     Bsdf bsdf;
                     const uint32_t mi = mflags & 0xffffu;
                     make_bsdf<MAT>(R->scene.materials[mi], R->scene.material_spectra + (size_t)mi * (5 * B200PT_NSPEC), is, &bsdf);
-                    SobolStream st;
-                    st.index = R->path[slot].sobol;
-                    st.dim = (int)(meta & 0xffffu);
-                    st.px = st.py = 0;
+                    SobolStream st = sobol_stream(P.sobol, v.meta);
                     const SamplerParams &sp = R->sampler;
                     if ((R->volpath || bsdf_num_components(bsdf, BSDF_ALL & ~BSDF_SPECULAR) > 0) && R->n_lights > 0) {
                         float pickPdf;
-                        const float *cdf = R->light_cdf, *func = R->light_func;
-                        float funcInt = R->light_func_int;
-                        if (R->grid.enabled) {
-                            const int vox = spatial_voxel(R->grid, is.p);
-                            cdf = R->sp_cdf + (size_t)vox * (R->n_lights + 1);
-                            func = R->sp_func + (size_t)vox * R->n_lights;
-                            funcInt = R->sp_func_int[vox];
-                        }
-                        const int lightNum = sample_discrete(cdf, func, funcInt, R->n_lights, get1d(sp, st), &pickPdf);
+                        const int lightNum = pick_light(R, is.p, get1d(sp, st), &pickPdf);
                         if (pickPdf != 0) {
                             float uLight[2], uScattering[2];
                             get2d(sp, st, uLight);
@@ -1914,7 +1923,7 @@ __global__ void __launch_bounds__(128, B200PT_S60_SHADE_MINCTAS) k_shade(const R
                         }
                     }
                     // path.cpp:131-150
-                    const V3 wo = -rd;
+                    const V3 wo = -v.rd;
                     V3 wi = mk(0.f, 0.f, 0.f);
                     float pdf = 0.f;
                     int flags = 0;
@@ -1926,7 +1935,7 @@ __global__ void __launch_bounds__(128, B200PT_S60_SHADE_MINCTAS) k_shade(const R
                         const bool spec = (flags & BSDF_SPECULAR) != 0;
                         if ((flags & BSDF_SPECULAR) && (flags & BSDF_TRANSMISSION)) {
                             const float eta = bsdf.eta;
-                            etaScale *= (dot(wo, is.n) > 0) ? (eta * eta) : 1 / (eta * eta);
+                            v.etaScale *= (dot(wo, is.n) > 0) ? (eta * eta) : 1 / (eta * eta);
                         }
                         const V3 no = offset_ray_origin(is.p, is.pError, is.n, wi);
                         cont = true;
@@ -1943,41 +1952,22 @@ __global__ void __launch_bounds__(128, B200PT_S60_SHADE_MINCTAS) k_shade(const R
                             for (int j = 0; j < 4; ++j) {
                                 const float nb = bold[j] * ((fv[j] * ad) / pdf);
                                 nbv[j] = nb;
-                                const float rr = nb * etaScale;
+                                const float rr = nb * v.etaScale;
                                 mx = (b0 + j == 0) ? rr : pt_max(mx, rr);
                             }
                             sBeta[b0 >> 2] = make_float4(nbv[0], nbv[1], nbv[2], nbv[3]);
                         }
-                        if (mx < R->rr_threshold && bounces > 3) {
-                            const float q = pt_max(.05f, 1 - mx);
-                            if (get1d(sp, st) < q)
-                                cont = false;
-                            else {
-                                const float dq = 1 - q;
-#pragma unroll 5
-                                for (int q = 0; q < B200PT_NSPEC / 4; ++q) {
-                                    const float4 v = sBeta[q];
-                                    sBeta[q] = make_float4(v.x / dq, v.y / dq, v.z / dq, v.w / dq);
-                                }
-                            }
-                        }
+                        if (mx < R->rr_threshold && v.bounces > 3) cont = russian_roulette(mx, get1d(sp, st), sBeta);
                         if (cont) {
-                            const uint32_t nmeta = ((uint32_t)st.dim & 0xffffu) | ((uint32_t)(bounces + 1) << 16) |
-                                                   ((spec ? (uint32_t)PF_SPECULAR : 0u) << 24);
-                            R->path[slot].o = f4(no, etaScale);
-                            R->path[slot].d = f4(wi, __uint_as_float(nmeta));
-                            R->path[slot].beta = make_float4(0.f, 0.f, 0.f, 0.f);
+                            P.o = f4(no, v.etaScale);
+                            P.d = f4(wi, __uint_as_float(pack_meta(st.dim, v.bounces + 1, spec)));
+                            P.beta = make_float4(0.f, 0.f, 0.f, 0.f);
                         }
                     }
                 }
             }
         }
-        const uint32_t ps = warp_append(qc_shadow, (pend & PEND_LIGHT) != 0);
-        if (pend & PEND_LIGHT) R->q_shadow[ps] = slot;
-        const uint32_t pm = warp_append(qc_mis, (pend & PEND_BSDF) != 0);
-        if (pend & PEND_BSDF) R->q_mis[pm] = slot;
-        const uint32_t pn = warp_append(qc_next, cont);
-        if (cont) q_next[pn] = slot;
+        append_vertex_out(R, qc, qc_next, q_next, pend, cont, slot);
     }
 }
 #endif  // B200PT_NSPEC == 3 (k_shade)
@@ -1996,11 +1986,9 @@ __global__ void __launch_bounds__(128, 4) k_medium(const RenderDev *R, int bounc
     uint32_t *q_next = R->q_path[(bounce + 1) & 1];
 #if B200PT_NSPEC == 3
     const Spec sigmaT = medium_sigma_t(R), sigmaS = medium_sigma_s(R);
-#define PT_SIGMA_T(ch_) sigmaT.c[ch_]
 #else
     // 60 bins: the medium's rows are read in place and beta is streamed through the slot's row (lazy spectra, see k_shade)
     const float *sigmaSrow = R->med_spectra, *sigmaTrow = R->med_spectra + B200PT_NSPEC;
-#define PT_SIGMA_T(ch_) sigmaTrow[ch_]
 #endif
     uint32_t i;
     while (warp_fetch(work, n, &i)) {
@@ -2010,63 +1998,32 @@ __global__ void __launch_bounds__(128, 4) k_medium(const RenderDev *R, int bounc
         uint32_t pend = 0, slot = 0;
         if (active) {
             slot = queue[i];
-            const float4 o4 = R->path[slot].o, d4 = R->path[slot].d;
+            PathRec &P = R->path[slot];
+            const PathVertex v = load_vertex(P);
 #if B200PT_NSPEC == 3
             float betaW;
-            Spec beta = ld_spec(R->path[slot].beta, R->s_beta, slot, &betaW);
+            Spec beta = ld_spec(P.beta, R->s_beta, slot, &betaW);
 #else
-            const float betaW = R->path[slot].beta.w;
+            const float betaW = P.beta.w;
             float4 *sBeta = reinterpret_cast<float4 *>(R->s_beta + (size_t)slot * B200PT_NSPEC);
 #endif
-            const V3 ro = v3(o4), rd = v3(d4);
-            const float etaScale = o4.w;
-            const uint32_t meta = __float_as_uint(d4.w);
-            const int bounces = (int)((meta >> 16) & 0xffu);
-            // distance of the closest hit (ray.tMax after Scene::Intersect) and its material
-            const uint32_t ti = R->path[slot].hit;
-            float tHit = pt_inf();
-            uint32_t mflags = 0;
-            if (ti != B200PT_MISS) {
-                if (is_sphere_hit(ti)) {
-                    const DevSphere *sp = R->scene.spheres + (ti & SPHERE_HIT_MASK);
-                    float th;
-                    if (sphere_intersect(*sp, ro, rd, pt_inf(), &th, nullptr)) tHit = th;
-                    mflags = sp->mat_flags;
-                } else {
-                    const F4 *tp = R->scene.tris + (size_t)ti * 3;
-                    const F4 t0 = ld_f4(tp), t1 = ld_f4(tp + 1), t2 = ld_f4(tp + 2);
-                    mflags = __float_as_uint(t1.w);
-                    V3 o2 = ro, d2 = rd;
-                    if (mflags & 0x100000u) {  // a triangle of an instanced object: same ray parameter in the object's space
-                        float tm2;
-                        instance_ray(R->scene.instances[R->path[slot].hit_inst], ro, rd, pt_inf(), &o2, &d2, &tm2);
-                    }
-                    TriHit h;
-                    if (triangle_test(v3(t0), v3(t1), v3(t2), o2, make_shear(d2), pt_inf(), &h)) tHit = h.t;
-                }
-            }
-            SobolStream st;
-            st.index = R->path[slot].sobol;
-            st.dim = (int)(meta & 0xffffu);
-            st.px = st.py = 0;
+            const uint32_t ti = P.hit;
+            uint32_t mflags;
+            const float tHit = hit_distance(R, P, ti, v.ro, v.rd, &mflags);
+            SobolStream st = sobol_stream(P.sobol, v.meta);
             const SamplerParams &sp = R->sampler;
             // HomogeneousMedium::Sample
-            const int channel = pt_mini((int)(get1d(sp, st) * B200PT_NSPEC), B200PT_NSPEC - 1);
-            const float dist = -pt_logf(1 - get1d(sp, st)) / PT_SIGMA_T(channel);
-            const float rdLen = len(rd);
-            const float t = pt_min(dist / rdLen, tHit);
-            const bool sampledMedium = t < tHit;
+            const float uChannel = get1d(sp, st), uDist = get1d(sp, st);
 #if B200PT_NSPEC == 3
-            Spec Tr;
-            PT_UNROLL SPEC_FOR Tr.c[i_] = pt_expf((-sigmaT.c[i_]) * pt_min(t, PT_MAX_FLOAT) * rdLen);
-            const Spec density = sampledMedium ? (sigmaT * Tr) : Tr;
-            float pdf = 0.f;
-            SPEC_FOR pdf += density.c[i_];
-            pdf *= 1 / (float)B200PT_NSPEC;
-            if (pdf == 0) pdf = 1;
-            beta = beta * (sampledMedium ? (Tr * sigmaS / pdf) : (Tr / pdf));
+            bool sampledMedium;
+            const float t = sample_medium_rgb(sigmaT, sigmaS, v.rd, tHit, uChannel, uDist, &beta, &sampledMedium);
             const bool alive = !is_black(beta);
 #else
+            const int channel = pt_mini((int)(uChannel * B200PT_NSPEC), B200PT_NSPEC - 1);
+            const float dist = -pt_logf(1 - uDist) / sigmaTrow[channel];
+            const float rdLen = len(v.rd);
+            const float t = pt_min(dist / rdLen, tHit);
+            const bool sampledMedium = t < tHit;
             // two passes over the bins: the pdf (mean density), then beta *= Tr [* sigma_s] / pdf with the is_black test
             const float tClamped = pt_min(t, PT_MAX_FLOAT);
             float pdf = 0.f;
@@ -2097,30 +2054,18 @@ __global__ void __launch_bounds__(128, 4) k_medium(const RenderDev *R, int bounc
                 if (!sampledMedium) {
                     // on to the surface vertex (or out of the scene)
 #if B200PT_NSPEC == 3
-                    st_spec(R->path[slot].beta, R->s_beta, slot, beta, betaW);
+                    st_spec(P.beta, R->s_beta, slot, beta, betaW);
 #else
-                    R->path[slot].beta = make_float4(0.f, 0.f, 0.f, betaW);
+                    P.beta = make_float4(0.f, 0.f, 0.f, betaW);
 #endif
-                    R->path[slot].d = f4(rd, __uint_as_float((meta & 0xffff0000u) | ((uint32_t)st.dim & 0xffffu)));
-                    if (ti != B200PT_MISS) family = R->scene.materials[mflags & 0xffffu].type;
-                } else if (bounces < R->max_depth) {  // volpath.cpp:84-85
-                    Isect mi;  // MediumInteraction(ray(t), -ray.d, ...): no normal, no error bounds
-                    mi.p = ro + rd * t;
-                    mi.wo = -rd;
-                    mi.n = mi.ns = mk(0.f, 0.f, 0.f);
-                    mi.pError = mk(0.f, 0.f, 0.f);
+                    P.d = f4(v.rd, __uint_as_float(meta_with_dim(v.meta, st.dim)));
+                    if (ti != B200PT_MISS) family = hit_family(R->scene.materials, mflags);
+                } else if (v.bounces < R->max_depth) {  // volpath.cpp:84-85
+                    const Isect mi = medium_interaction(v.ro, v.rd, t);
                     if (R->n_lights > 0) {
                         // UniformSampleOneLight(mi, ..., handleMedia = true), integrator.cpp:85-106
                         float pickPdf;
-                        const float *cdf = R->light_cdf, *func = R->light_func;
-                        float funcInt = R->light_func_int;
-                        if (R->grid.enabled) {
-                            const int vox = spatial_voxel(R->grid, mi.p);
-                            cdf = R->sp_cdf + (size_t)vox * (R->n_lights + 1);
-                            func = R->sp_func + (size_t)vox * R->n_lights;
-                            funcInt = R->sp_func_int[vox];
-                        }
-                        const int lightNum = sample_discrete(cdf, func, funcInt, R->n_lights, get1d(sp, st), &pickPdf);
+                        const int lightNum = pick_light(R, mi.p, get1d(sp, st), &pickPdf);
                         if (pickPdf != 0) {
                             float uLight[2], uScattering[2];
                             get2d(sp, st, uLight);
@@ -2171,90 +2116,40 @@ __global__ void __launch_bounds__(128, 4) k_medium(const RenderDev *R, int bounc
                     const V3 no = offset_ray_origin(mi.p, mi.pError, mi.n, wi);
                     cont = true;
 #if B200PT_NSPEC == 3
-                    const Spec rrBeta = beta * etaScale;  // volpath.cpp:176-184
-                    if (max_comp(rrBeta) < R->rr_threshold && bounces > 3) {
-                        const float q = pt_max(.05f, 1 - max_comp(rrBeta));
-                        if (get1d(sp, st) < q)
-                            cont = false;
-                        else
-                            beta = beta / (1 - q);
-                    }
+                    const float rrMax = max_comp(beta * v.etaScale);  // volpath.cpp:176-184
+                    if (rrMax < R->rr_threshold && v.bounces > 3) cont = russian_roulette(rrMax, get1d(sp, st), &beta);
 #else
-                    if (bounces > 3) {  // volpath.cpp:176-184 (the maximum is only needed then)
+                    if (v.bounces > 3) {  // volpath.cpp:176-184 (the maximum is only needed then)
                         float mx = 0.f;
 #pragma unroll 3
                         for (int q4 = 0; q4 < B200PT_NSPEC / 4; ++q4) {
-                            const float4 v = sBeta[q4];
-                            const float r0 = v.x * etaScale, r1 = v.y * etaScale, r2 = v.z * etaScale, r3 = v.w * etaScale;
+                            const float4 b = sBeta[q4];
+                            const float r0 = b.x * v.etaScale, r1 = b.y * v.etaScale, r2 = b.z * v.etaScale, r3 = b.w * v.etaScale;
                             mx = q4 == 0 ? r0 : pt_max(mx, r0);
                             mx = pt_max(pt_max(pt_max(mx, r1), r2), r3);
                         }
-                        if (mx < R->rr_threshold) {
-                            const float q = pt_max(.05f, 1 - mx);
-                            if (get1d(sp, st) < q)
-                                cont = false;
-                            else {
-                                const float dq = 1 - q;
-#pragma unroll 5
-                                for (int q4 = 0; q4 < B200PT_NSPEC / 4; ++q4) {
-                                    const float4 v = sBeta[q4];
-                                    sBeta[q4] = make_float4(v.x / dq, v.y / dq, v.z / dq, v.w / dq);
-                                }
-                            }
-                        }
+                        if (mx < R->rr_threshold) cont = russian_roulette(mx, get1d(sp, st), sBeta);
                     }
 #endif
                     if (cont) {
-                        const uint32_t nmeta = ((uint32_t)st.dim & 0xffffu) | ((uint32_t)(bounces + 1) << 16);  // specularBounce = false
-                        R->path[slot].o = f4(no, etaScale);
-                        R->path[slot].d = f4(wi, __uint_as_float(nmeta));
+                        P.o = f4(no, v.etaScale);
+                        P.d = f4(wi, __uint_as_float(pack_meta(st.dim, v.bounces + 1, false)));
 #if B200PT_NSPEC == 3
-                        st_spec(R->path[slot].beta, R->s_beta, slot, beta, 0.f);
+                        st_spec(P.beta, R->s_beta, slot, beta, 0.f);
 #else
-                        R->path[slot].beta = make_float4(0.f, 0.f, 0.f, 0.f);
+                        P.beta = make_float4(0.f, 0.f, 0.f, 0.f);
 #endif
                     }
                 }
             }
         }
-#pragma unroll
-        for (int m = 0; m < 4; ++m) {
-            const bool mine = family == m;
-            const uint32_t pos = warp_append(&qc[Q_MAT0 + m], mine);
-            if (mine) R->q_mat[m][pos] = slot;
-        }
-        const uint32_t ps = warp_append(&qc[Q_SHADOW], (pend & PEND_LIGHT) != 0);
-        if (pend & PEND_LIGHT) R->q_shadow[ps] = slot;
-        const uint32_t pm = warp_append(&qc[Q_MIS], (pend & PEND_BSDF) != 0);
-        if (pend & PEND_BSDF) R->q_mis[pm] = slot;
-        const uint32_t pn = warp_append(qc_next, cont);
-        if (cont) q_next[pn] = slot;
+        append_family(R->q_mat, &qc[Q_MAT0], family, slot);
+        append_vertex_out(R, qc, qc_next, q_next, pend, cont, slot);
     }
 }
-#undef PT_SIGMA_T
 
 #if B200PT_MEDIA_GENERAL
 // ---- media bounded by null-material spheres (b200pt_integrator_desc::bounded_media) ------------------------------------
-// distance of the closest hit `ti` along (ro, rd) -- ray.tMax after Scene::Intersect -- and the hit's material word
-// (render_create refuses bounded media in scenes with object instances)
-__device__ __forceinline__ float hit_distance(const RenderDev *R, uint32_t ti, const V3 &ro, const V3 &rd, uint32_t *mflags) {
-    float tHit = pt_inf();
-    *mflags = 0;
-    if (ti == B200PT_MISS) return tHit;
-    if (is_sphere_hit(ti)) {
-        const DevSphere *sp = R->scene.spheres + (ti & SPHERE_HIT_MASK);
-        float th;
-        if (sphere_intersect(*sp, ro, rd, pt_inf(), &th, nullptr)) tHit = th;
-        *mflags = sp->mat_flags;
-    } else {
-        const F4 *tp = R->scene.tris + (size_t)ti * 3;
-        const F4 t0 = ld_f4(tp), t1 = ld_f4(tp + 1), t2 = ld_f4(tp + 2);
-        *mflags = __float_as_uint(t1.w);
-        TriHit h;
-        if (triangle_test(v3(t0), v3(t1), v3(t2), ro, make_shear(rd), pt_inf(), &h)) tHit = h.t;
-    }
-    return tHit;
-}
 // medium id inside the boundary sphere that hit `ti` names, -1 when the hit is an ordinary surface (or a miss)
 __device__ __forceinline__ int boundary_medium(const RenderDev *R, uint32_t ti) {
     return (ti != B200PT_MISS && is_sphere_hit(ti)) ? R->sphere_med[ti & SPHERE_HIT_MASK] : -1;
@@ -2280,22 +2175,16 @@ __global__ void __launch_bounds__(128, 4) k_medium_general(const RenderDev *R, i
         uint32_t pend = 0, slot = 0;
         if (active) {
             slot = queue[i];
-            const float4 o4 = R->path[slot].o, d4 = R->path[slot].d;
+            PathRec &P = R->path[slot];
+            const PathVertex v = load_vertex(P);
             float betaW;
-            Spec beta = ld_spec(R->path[slot].beta, R->s_beta, slot, &betaW);
-            const V3 ro = v3(o4), rd = v3(d4);
-            const float etaScale = o4.w;
-            const uint32_t meta = __float_as_uint(d4.w);
-            const int bounces = (int)((meta >> 16) & 0xffu);
+            Spec beta = ld_spec(P.beta, R->s_beta, slot, &betaW);
             const int med = R->cur_med[slot];
-            const uint32_t ti = R->path[slot].hit;
+            const uint32_t ti = P.hit;
             uint32_t mflags;
-            const float tHit = hit_distance(R, ti, ro, rd, &mflags);
+            const float tHit = hit_distance(R, P, ti, v.ro, v.rd, &mflags);
             const int bm = boundary_medium(R, ti);
-            SobolStream st;
-            st.index = R->path[slot].sobol;
-            st.dim = (int)(meta & 0xffffu);
-            st.px = st.py = 0;
+            SobolStream st = sobol_stream(P.sobol, v.meta);
             const SamplerParams &sp = R->sampler;
             // every boundary crossed inside a medium spends two dimensions, so a path can run past the host's tables (the
             // reference aborts there, sobol.cpp / lowdiscrepancy.h:229); such a path ends here and is counted
@@ -2307,61 +2196,37 @@ __global__ void __launch_bounds__(128, 4) k_medium_general(const RenderDev *R, i
             bool sampledMedium = false;
             float t = tHit;
             if (alive && med >= 0) {  // ray.medium->Sample (homogeneous.cpp:49-76)
-                const Spec sigmaT = media_sigma_t(R, med), sigmaS = media_sigma_s(R, med);
-                const int channel = pt_mini((int)(get1d(sp, st) * B200PT_NSPEC), B200PT_NSPEC - 1);
-                const float dist = -pt_logf(1 - get1d(sp, st)) / sigmaT.c[channel];
-                const float rdLen = len(rd);
-                t = pt_min(dist / rdLen, tHit);
-                sampledMedium = t < tHit;
-                Spec Tr;
-                PT_UNROLL SPEC_FOR Tr.c[i_] = pt_expf((-sigmaT.c[i_]) * pt_min(t, PT_MAX_FLOAT) * rdLen);
-                const Spec density = sampledMedium ? (sigmaT * Tr) : Tr;
-                float pdf = 0.f;
-                SPEC_FOR pdf += density.c[i_];
-                pdf *= 1 / (float)B200PT_NSPEC;
-                if (pdf == 0) pdf = 1;
-                beta = beta * (sampledMedium ? (Tr * sigmaS / pdf) : (Tr / pdf));
+                const float uChannel = get1d(sp, st), uDist = get1d(sp, st);
+                t = sample_medium_rgb(media_sigma_t(R, med), media_sigma_s(R, med), v.rd, tHit, uChannel, uDist, &beta, &sampledMedium);
             }
             if (alive && !is_black(beta)) {
                 if (!sampledMedium) {
                     if (bm >= 0) {
                         // a medium boundary: nothing is emitted or scattered there; volpath.cpp:112 ends the path at maxDepth
-                        if (bounces < R->max_depth) {
+                        if (v.bounces < R->max_depth) {
                             const DevSphere *bs = R->scene.spheres + (ti & SPHERE_HIT_MASK);
                             float th;
                             Isect is;
-                            if (sphere_intersect(*bs, ro, rd, pt_inf(), &th, &is)) {
-                                R->cur_med[slot] = dot(rd, is.n) > 0 ? outside : bm;          // GetMedium(ray.d)
-                                const V3 no = offset_ray_origin(is.p, is.pError, is.n, rd);  // isect.SpawnRay(ray.d)
-                                R->path[slot].o = f4(no, etaScale);
-                                R->path[slot].d = f4(rd, __uint_as_float((meta & 0xffff0000u) | ((uint32_t)st.dim & 0xffffu)));
-                                st_spec(R->path[slot].beta, R->s_beta, slot, beta, betaW);
+                            if (sphere_intersect(*bs, v.ro, v.rd, pt_inf(), &th, &is)) {
+                                R->cur_med[slot] = dot(v.rd, is.n) > 0 ? outside : bm;          // GetMedium(ray.d)
+                                const V3 no = offset_ray_origin(is.p, is.pError, is.n, v.rd);  // isect.SpawnRay(ray.d)
+                                P.o = f4(no, v.etaScale);
+                                P.d = f4(v.rd, __uint_as_float(meta_with_dim(v.meta, st.dim)));
+                                st_spec(P.beta, R->s_beta, slot, beta, betaW);
                                 cross = true;
                             }
                         }
                     } else {
                         // on to the surface vertex (or out of the scene)
-                        st_spec(R->path[slot].beta, R->s_beta, slot, beta, betaW);
-                        R->path[slot].d = f4(rd, __uint_as_float((meta & 0xffff0000u) | ((uint32_t)st.dim & 0xffffu)));
-                        if (ti != B200PT_MISS) family = R->scene.materials[mflags & 0xffffu].type;
+                        st_spec(P.beta, R->s_beta, slot, beta, betaW);
+                        P.d = f4(v.rd, __uint_as_float(meta_with_dim(v.meta, st.dim)));
+                        if (ti != B200PT_MISS) family = hit_family(R->scene.materials, mflags);
                     }
-                } else if (bounces < R->max_depth) {  // volpath.cpp:84-85
-                    Isect mi;  // MediumInteraction(ray(t), -ray.d, ...): no normal, no error bounds
-                    mi.p = ro + rd * t;
-                    mi.wo = -rd;
-                    mi.n = mi.ns = mk(0.f, 0.f, 0.f);
-                    mi.pError = mk(0.f, 0.f, 0.f);
+                } else if (v.bounces < R->max_depth) {  // volpath.cpp:84-85
+                    const Isect mi = medium_interaction(v.ro, v.rd, t);
                     if (R->n_lights > 0) {
                         float pickPdf;
-                        const float *cdf = R->light_cdf, *func = R->light_func;
-                        float funcInt = R->light_func_int;
-                        if (R->grid.enabled) {
-                            const int vox = spatial_voxel(R->grid, mi.p);
-                            cdf = R->sp_cdf + (size_t)vox * (R->n_lights + 1);
-                            func = R->sp_func + (size_t)vox * R->n_lights;
-                            funcInt = R->sp_func_int[vox];
-                        }
-                        const int lightNum = sample_discrete(cdf, func, funcInt, R->n_lights, get1d(sp, st), &pickPdf);
+                        const int lightNum = pick_light(R, mi.p, get1d(sp, st), &pickPdf);
                         if (pickPdf != 0) {
                             float uLight[2], uScattering[2];
                             get2d(sp, st, uLight);
@@ -2391,35 +2256,18 @@ __global__ void __launch_bounds__(128, 4) k_medium_general(const RenderDev *R, i
                     hg_sample_p(R->media_g[med], mi.wo, &wi, u2);
                     const V3 no = offset_ray_origin(mi.p, mi.pError, mi.n, wi);
                     cont = true;
-                    const Spec rrBeta = beta * etaScale;  // volpath.cpp:176-184
-                    if (max_comp(rrBeta) < R->rr_threshold && bounces > 3) {
-                        const float q = pt_max(.05f, 1 - max_comp(rrBeta));
-                        if (get1d(sp, st) < q)
-                            cont = false;
-                        else
-                            beta = beta / (1 - q);
-                    }
+                    const float rrMax = max_comp(beta * v.etaScale);  // volpath.cpp:176-184
+                    if (rrMax < R->rr_threshold && v.bounces > 3) cont = russian_roulette(rrMax, get1d(sp, st), &beta);
                     if (cont) {
-                        const uint32_t nmeta = ((uint32_t)st.dim & 0xffffu) | ((uint32_t)(bounces + 1) << 16);  // specularBounce = false
-                        R->path[slot].o = f4(no, etaScale);
-                        R->path[slot].d = f4(wi, __uint_as_float(nmeta));
-                        st_spec(R->path[slot].beta, R->s_beta, slot, beta, 0.f);
+                        P.o = f4(no, v.etaScale);
+                        P.d = f4(wi, __uint_as_float(pack_meta(st.dim, v.bounces + 1, false)));
+                        st_spec(P.beta, R->s_beta, slot, beta, 0.f);
                     }
                 }
             }
         }
-#pragma unroll
-        for (int m = 0; m < 4; ++m) {
-            const bool mine = family == m;
-            const uint32_t pos = warp_append(&qc[Q_MAT0 + m], mine);
-            if (mine) R->q_mat[m][pos] = slot;
-        }
-        const uint32_t ps = warp_append(&qc[Q_SHADOW], (pend & PEND_LIGHT) != 0);
-        if (pend & PEND_LIGHT) R->q_shadow[ps] = slot;
-        const uint32_t pm = warp_append(&qc[Q_MIS], (pend & PEND_BSDF) != 0);
-        if (pend & PEND_BSDF) R->q_mis[pm] = slot;
-        const uint32_t pn = warp_append(qc_next, cont);
-        if (cont) q_next[pn] = slot;
+        append_family(R->q_mat, &qc[Q_MAT0], family, slot);
+        append_vertex_out(R, qc, qc_next, q_next, pend, cont, slot);
         const uint32_t pc = warp_append(cross_count, cross);
         if (cross) q_cross[pc] = slot;
     }
@@ -2515,7 +2363,7 @@ __global__ void __launch_bounds__(128, 4) k_direct_walk(const RenderDev *R, cons
                                 TriShading lsh;
                                 load_shading<true>(R->scene, ti, lflags, &lsh);
                                 Isect li;
-                                fill_isect(v3(t0), v3(t1), v3(t2), (lflags & 0x10000u) != 0, lsh, h, wi, &li);
+                                fill_isect(v3(t0), v3(t1), v3(t2), (lflags & B200PT_TRI_FLIP) != 0, lsh, h, wi, &li);
                                 ln = li.n;
                                 t = h.t;
                             }
@@ -2658,7 +2506,7 @@ __global__ void __launch_bounds__(128) k_spatial_contrib(const RenderDev *R) {
     TriShading lsh;
     load_shading<true>(R->scene, isDelta ? 0u : light.tri, lflags, &lsh);
     R->sp_func[vox * R->n_lights + j] =
-        spatial_light_contrib(g, vx, vy, vz, v3(t0), v3(t1), v3(t2), (lflags & 0x10000u) != 0, lsh, lemit,
+        spatial_light_contrib(g, vx, vy, vz, v3(t0), v3(t1), v3(t2), (lflags & B200PT_TRI_FLIP) != 0, lsh, lemit,
                               light.two_sided != 0, onSphere ? R->scene.spheres + (light.tri & SPHERE_HIT_MASK) : nullptr,
                               isDelta ? &dl : nullptr);
 }

@@ -53,6 +53,28 @@ struct DevScene {
 
 // queue ids inside one bounce's counter block
 enum { Q_PATH = 0, Q_MAT0 = 1, Q_SHADOW = 5, Q_MIS = 6, Q_NEXT = 7, Q_PER_BOUNCE = 8 };
+// persistent-fetch counters (RenderDev::work) inside one bounce's block: one per launch of the bounce
+enum {
+    W_TRACE_PATH = 0,      // closest hit of the path rays
+    W_SHADE0 = 1,          // k_shade of BSDF family m: W_SHADE0 + m
+    W_TRACE_SHADOW = 5,
+    W_TRACE_MIS = 6,
+    W_RESOLVE = 7,
+    W_SPHERES_PATH = 8,    // the sphere passes behind the three traversal launches
+    W_SPHERES_SHADOW = 9,
+    W_SPHERES_MIS = 10,
+    W_MEDIUM = 11,
+    W_PER_BOUNCE = 16
+};
+// bounded media: the counters of the boundary passes inside a bounce (zeroed between passes, see b200pt_render_tiles)
+enum {
+    WC_CROSS0 = 0,  // rays that crossed a boundary in this pass / the one before (ping-pong)
+    WC_CROSS1 = 1,
+    WC_WALK = 2,    // fetch counters of the pass's medium or walk kernel, its traversal launch and its sphere pass
+    WC_TRACE = 3,
+    WC_SPHERES = 4,
+    WC_COUNT = 16
+};
 // meta word of a path: dim (16 bits) | bounces (8) | flags (8)
 enum { PF_SPECULAR = 1 };
 // pending direct-lighting flags
@@ -138,7 +160,7 @@ struct RenderDev {
     uint32_t *q_shadow;
     uint32_t *q_mis;
     uint32_t *qcount;          // [(max_depth + 2) * Q_PER_BOUNCE]
-    uint32_t *work;            // persistent-fetch counters, one per launch of a batch
+    uint32_t *work;            // [(max_depth + 2) * W_PER_BOUNCE] persistent-fetch counters, one per launch of a batch
     unsigned long long *stats; // camera, regular, shadow, nodes, tris
     // VolPathIntegrator (b200pt_integrator_desc::volumetric / medium): light sampling at every vertex; with has_medium
     // every ray is inside one homogeneous medium (RGB build only)
@@ -148,7 +170,7 @@ struct RenderDev {
     // Media bounded by null-material spheres (b200pt_integrator_desc::bounded_media, RGB build): medium ids are -1 = vacuum,
     // 0 = the medium around the scene, k >= 1 = bounded_media[k - 1].  The path ray's medium is per-slot state; rays that
     // reach a boundary are traced again from the far side within the same bounce (q_cross), shadow and MIS rays walk from
-    // boundary to boundary while their transmittance accumulates (k_shadow_walk / k_mis_walk).
+    // boundary to boundary while their transmittance accumulates (k_direct_walk<shadow>).
     int med_general;
     const float *media_tab;    // [1 + n_bounded][2][3] = sigma_s, sigma_t of medium id k
     const float *media_g;      // [1 + n_bounded]

@@ -369,8 +369,9 @@ B200_HD void lbvh_collapse(const LbvhCtx &c, const LbvhItem &it) {
                 }
                 const uint8_t vf = c.vertex_flags ? c.vertex_flags[tri] : 3;
                 r.prim = tri;
-                r.mat_flags = (uint32_t)(c.material_id ? c.material_id[tri] : 0) | ((c.flip && c.flip[tri]) ? 0x10000u : 0u) |
-                              ((c.has_normals && (vf & 1)) ? 0x40000u : 0u) | ((c.has_uvs && (vf & 2)) ? 0x80000u : 0u);
+                r.mat_flags = (uint32_t)(c.material_id ? c.material_id[tri] : 0) | ((c.flip && c.flip[tri]) ? B200PT_TRI_FLIP : 0u) |
+                              ((c.has_normals && (vf & 1)) ? B200PT_TRI_HAS_NORMALS : 0u) |
+                              ((c.has_uvs && (vf & 2)) ? B200PT_TRI_HAS_UVS : 0u);
                 r.light = c.light_id ? c.light_id[tri] : -1;
                 c.tris[pos] = r;
                 c.prim_to_tri[tri] = pos;
@@ -403,8 +404,9 @@ B200_HD void lbvh_leftover(const LbvhCtx &c, int64_t i) {
     }
     const uint8_t vf = c.vertex_flags ? c.vertex_flags[i] : 3;
     r.prim = (uint32_t)i;
-    r.mat_flags = (uint32_t)(c.material_id ? c.material_id[i] : 0) | ((c.flip && c.flip[i]) ? 0x10000u : 0u) | 0x20000u |
-                  ((c.has_normals && (vf & 1)) ? 0x40000u : 0u) | ((c.has_uvs && (vf & 2)) ? 0x80000u : 0u);
+    r.mat_flags = (uint32_t)(c.material_id ? c.material_id[i] : 0) | ((c.flip && c.flip[i]) ? B200PT_TRI_FLIP : 0u) |
+                  B200PT_TRI_DEGENERATE | ((c.has_normals && (vf & 1)) ? B200PT_TRI_HAS_NORMALS : 0u) |
+                  ((c.has_uvs && (vf & 2)) ? B200PT_TRI_HAS_UVS : 0u);
     r.light = c.light_id ? c.light_id[i] : -1;
     c.tris[pos] = r;
     c.prim_to_tri[i] = pos;

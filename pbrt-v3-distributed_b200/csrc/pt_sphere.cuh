@@ -21,6 +21,7 @@
 
 #include "pt_core.cuh"
 #include "pt_sincos.cuh"
+#include "wbvh.h"
 
 namespace B200PT_NS {
 
@@ -36,7 +37,7 @@ struct DevSphere {
     float theta_min, theta_max;  // Sphere::thetaMin / thetaMax; acos(-1), acos(1) for a full sphere
     float z_min, z_max;      // Sphere::zMin / zMax; -r, r for a full sphere
     float area;              // Sphere::Area(), sphere.cpp:207
-    uint32_t mat_flags;      // material id | flip << 16 (reverseOrientation ^ transformSwapsHandedness)
+    uint32_t mat_flags;      // material id | B200PT_TRI_FLIP (reverseOrientation ^ transformSwapsHandedness)
     int light_id;
     int reverse_orientation;
     float leaf_lo[3], leaf_hi[3];  // bounds of the host accelerator's leaf holding the sphere (b200pt_sphere::leaf_bounds)
@@ -354,7 +355,7 @@ B200_HD bool sphere_intersect(const DevSphere &sp, const V3 &ro, const V3 &rd, f
     const V3 dpdv = (sp.theta_max - sp.theta_min) * mk(pHit.z * cosPhi, pHit.z * sinPhi, -radius * pt_sinf(theta));
     const V3 pError = pt_gamma(5) * vabs(pHit);
     V3 n = normalize(cross(dpdu, dpdv));  // interaction.cpp:44-72
-    if (sp.mat_flags & 0x10000u) n = n * -1.f;
+    if (sp.mat_flags & B200PT_TRI_FLIP) n = n * -1.f;
     const V3 wo = normalize(-d);
     is->p = xform_point_err_in(sp.o2w, pHit, pError, &is->pError);  // transform.cpp:262-297
     is->n = normalize(xform_normal(sp.w2o, n));

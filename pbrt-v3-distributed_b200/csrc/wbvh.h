@@ -57,11 +57,18 @@ struct alignas(64) WbvhNode {
 };
 static_assert(sizeof(WbvhNode) == 64, "WbvhNode must be 64 bytes");
 
+// flag bits of TriRecord::mat_flags above the 16-bit material id (DevSphere::mat_flags has the flip bit only)
+#define B200PT_TRI_FLIP 0x10000u         // the geometric normal is flipped (reverseOrientation ^ transformSwapsHandedness)
+#define B200PT_TRI_DEGENERATE 0x20000u   // Triangle::Intersect rejects it
+#define B200PT_TRI_HAS_NORMALS 0x40000u  // per-vertex shading normals in DevScene::tri_n
+#define B200PT_TRI_HAS_UVS 0x80000u      // uvs in DevScene::tri_uv
+#define B200PT_TRI_INSTANCED 0x100000u   // object-space triangle of an instanced object
+
 struct alignas(16) TriRecord {  // 48 bytes
     float p0[3];
     uint32_t prim;
     float p1[3];
-    uint32_t mat_flags;  // material id | (flip_normal << 16) | (degenerate << 17) | normals << 18 | uvs << 19 | object-space << 20
+    uint32_t mat_flags;  // material id | B200PT_TRI_* flags
     float p2[3];
     int32_t light;
 };

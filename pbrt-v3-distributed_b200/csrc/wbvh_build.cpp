@@ -210,8 +210,8 @@ void build_wbvh(const float *vertices, int64_t n_tris, const int32_t *material_i
         memcpy(t.p1, v + 3, 12);
         memcpy(t.p2, v + 6, 12);
         t.prim = (uint32_t)i;
-        t.mat_flags = (uint32_t)(material_id ? material_id[i] : 0) | ((flip && flip[i]) ? 0x10000u : 0u) |
-                      ((degenerate && degenerate[i]) ? 0x20000u : 0u);
+        t.mat_flags = (uint32_t)(material_id ? material_id[i] : 0) | ((flip && flip[i]) ? B200PT_TRI_FLIP : 0u) |
+                      ((degenerate && degenerate[i]) ? B200PT_TRI_DEGENERATE : 0u);
         t.light = light_id ? light_id[i] : -1;
         return t;
     };
