@@ -16,6 +16,7 @@
 #include "pt_platform.h"
 #include "pt_sincos.cuh"
 #include "pt_explog.cuh"
+#include "pt_sincos_dbl.cuh"
 
 namespace B200PT_NS {
 
@@ -770,13 +771,14 @@ B200_HD float tr_pdf(const TRDist &d, const V3 &wo, const V3 &wh) {
     return tr_D(d, wh) * tr_G1(d, wo) * absdot(wo, wh) / abs_cos_theta(wo);
 }
 // microfacet.cpp:238-283.  The normal-incidence branch calls the C `cos`/`sin`
-// on a float (promoted to double) and multiplies in double.
+// on a float (promoted to double) and multiplies in double; pt_cos / pt_sin
+// (pt_sincos_dbl.cuh) round like the host's glibc, which libdevice's do not.
 B200_HD_L2 void tr_sample11(float cosTheta, float U1, float U2, float *slope_x, float *slope_y) {
     if ((double)cosTheta > .9999) {
         float r = sqrtf(U1 / (1 - U1));
         float phi = (float)(6.28318530718 * (double)U2);
-        *slope_x = (float)((double)r * cos((double)phi));
-        *slope_y = (float)((double)r * sin((double)phi));
+        *slope_x = (float)((double)r * pt_cos((double)phi));
+        *slope_y = (float)((double)r * pt_sin((double)phi));
         return;
     }
     float sinTheta = sqrtf(pt_max(0.f, 1.f - cosTheta * cosTheta));
