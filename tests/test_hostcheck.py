@@ -123,6 +123,16 @@ def test_host_logic_shards_batches_edges(hostcheck, abi, scenes, hctx, monkeypat
     G.test_render_is_deterministic_and_batch_independent(hostcheck, abi, scenes, hctx, monkeypatch)
 
 
+def test_fullsize_checks_at_a_small_film(hostcheck, abi, scenes, ob, hctx, monkeypatch):
+    """The benchmark-size tests (tests/test_zz_fullsize_gpu.py) at 160x90 with 7 tiles per batch: nine batches, a partial
+    last one, half-height bottom tiles -- the tile set, masks, launch-count arithmetic and comparisons on the CPU."""
+    import test_zz_fullsize_gpu as F
+    F.test_fullsize_rgb_cfg4_shape(hostcheck, abi, scenes, ob, hctx, monkeypatch, film=(160, 90, 16), n_tris=20000, batch_tiles=7)
+    F.test_fullsize_spectral_cfg5_shape(hostcheck, abi, scenes, ob, hctx, monkeypatch, film=(160, 90, 8), n_tris=2000, batch_tiles=7)
+    F.test_fullsize_volpath_cfg2fog_shape(hostcheck, abi, scenes, ob, hctx, monkeypatch, film=(160, 90, 16), n_tris=20000,
+                                          batch_tiles=7)
+
+
 def test_device_bvh_builder_is_refused(hostcheck, abi, scenes, hctx):
     """The check build has no device BVH builder; asking for it must fail loudly, not fall back to the host builder."""
     arr = scenes.SceneArrays(500, materials=("matte",), soup_version=1)
