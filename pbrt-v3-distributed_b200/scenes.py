@@ -188,7 +188,8 @@ class SceneArrays:
         self.two_sided = bool(two_sided)
         self._materials = None
         # object instancing: objects = dicts {n_tris, seed, material, size}; each is a small soup in its own space
-        # (written as ObjectBegin/ObjectEnd at the identity CTM); instances = dicts {object, center, scale}
+        # (written as ObjectBegin/ObjectEnd at the identity CTM); instances = dicts {object, center, scale, rotate,
+        # order} (instance_steps)
         self.n_toplevel = len(self.vertices)
         self.object_specs = [dict(o) for o in objects]
         self.instance_specs = [dict(i) for i in instances]
@@ -208,11 +209,10 @@ class SceneArrays:
             first, count = self.object_ranges[ins["object"]]
             rec = self._instances[k]
             rec.first_triangle, rec.n_triangles = first, count
-            ident = tuple(ins.get("center", (0, 0, 0))) == (0, 0, 0) and not ins.get("scale")
-            m, minv = sphere_transform(ins.get("center", (0, 0, 0)), ins.get("scale"))
+            m, minv = ctm(instance_steps(ins))
             rec.instance_to_world[:] = m.reshape(-1).tolist()
             rec.world_to_instance[:] = minv.reshape(-1).tolist()
-            rec.is_identity = int(ident)
+            rec.is_identity = int(np.array_equal(m, np.eye(4)))  # Transform::IsIdentity (transform.h:148-155)
         self.sphere_specs = [dict(s) for s in spheres]
         n_sl = sum(1 for s in self.sphere_specs if s.get("emit"))
         # delta lights: dicts {kind: "point"|"spot"|"distant", from_, to, I or L, coneangle, conedelta}; they follow
@@ -349,25 +349,68 @@ def _mat_mul(a, b):
     return r
 
 
-def sphere_transform(center, scale=None):
-    """CTM pbrt builds for `Translate c` [+ `Scale s`] inside an attribute block at identity
-    (api.cpp pbrtTranslate / pbrtScale: ctm = ctm * T; Transform::operator*, transform.cpp:222-225)."""
+def _libm_float(name):
+    """sinf / cosf of the host libm: what std::sin / std::cos of a float call in the reference."""
+    import ctypes.util
+    fn = getattr(C.CDLL(ctypes.util.find_library("m")), name)
+    fn.restype, fn.argtypes = C.c_float, [C.c_float]
+    return lambda x: np.float32(fn(float(x)))
+
+
+def step_transform(op, args):
+    """(m, mInv) of one CTM statement: Translate / Scale / Rotate (transform.cpp:141-153, :178-201).  Rotate restates
+    Normalize (geometry.h:984-986), Radians (pbrt.h:320) and the float sin / cos of the host libm; its inverse is the
+    transpose."""
     f = np.float32
     m = np.eye(4, dtype=f)
     minv = np.eye(4, dtype=f)
-    t = np.eye(4, dtype=f)
-    ti = np.eye(4, dtype=f)
-    t[:3, 3] = [f(c) for c in center]
-    ti[:3, 3] = [-f(c) for c in center]
-    m, minv = _mat_mul(m, t), _mat_mul(ti, minv)
-    if scale:
-        s_ = np.eye(4, dtype=f)
-        si = np.eye(4, dtype=f)
+    if op == "Translate":
+        m[:3, 3] = [f(c) for c in args]
+        minv[:3, 3] = [-f(c) for c in args]
+    elif op == "Scale":
         for a in range(3):
-            s_[a, a] = f(scale[a])
-            si[a, a] = f(1) / f(scale[a])
-        m, minv = _mat_mul(m, s_), _mat_mul(si, minv)
+            m[a, a] = f(args[a])
+            minv[a, a] = f(1) / f(args[a])
+    elif op == "Rotate":
+        v = [f(c) for c in args[1:]]
+        inv = f(1) / np.sqrt(f(f(f(v[0] * v[0]) + f(v[1] * v[1])) + f(v[2] * v[2])))
+        x, y, z = (f(c * inv) for c in v)
+        theta = f(f(f(3.14159265358979323846) / f(180)) * f(args[0]))
+        s, c = _libm_float("sinf")(theta), _libm_float("cosf")(theta)
+        omc = f(1 - c)
+        m[:3, :3] = [[f(f(x * x) + f(f(1 - f(x * x)) * c)), f(f(f(x * y) * omc) - f(z * s)), f(f(f(x * z) * omc) + f(y * s))],
+                     [f(f(f(x * y) * omc) + f(z * s)), f(f(y * y) + f(f(1 - f(y * y)) * c)), f(f(f(y * z) * omc) - f(x * s))],
+                     [f(f(f(x * z) * omc) - f(y * s)), f(f(f(y * z) * omc) + f(x * s)), f(f(z * z) + f(f(1 - f(z * z)) * c))]]
+        minv = np.ascontiguousarray(m.T)
+    else:
+        raise ValueError(op)
     return m, minv
+
+
+def ctm(steps):
+    """CTM pbrt builds from CTM statements inside an attribute block at identity (api.cpp pbrtTranslate / pbrtScale /
+    pbrtRotate: ctm = ctm * T; Transform::operator*, transform.cpp:222-225: the inverse multiplies in reverse order)."""
+    m = np.eye(4, dtype=np.float32)
+    minv = np.eye(4, dtype=np.float32)
+    for op, args in steps:
+        t, ti = step_transform(op, args)
+        m, minv = _mat_mul(m, t), _mat_mul(ti, minv)
+    return m, minv
+
+
+def sphere_transform(center, scale=None):
+    """CTM of `Translate c` [+ `Scale s`]."""
+    return ctm([("Translate", center)] + ([("Scale", scale)] if scale else []))
+
+
+def instance_steps(ins):
+    """The CTM statements of an instance spec, in the spec's `order` (default "TSR"): Translate `center`, Scale `scale`,
+    Rotate `rotate` = (degrees, ax, ay, az).  "TSR" gives the linear part S R (not orthogonal under a non-uniform
+    scale), "TRS" R S.  An instance with neither scale nor rotation nor offset has no statement (the identity)."""
+    c, sc, rot = tuple(ins.get("center", (0, 0, 0))), ins.get("scale"), ins.get("rotate")
+    have = {"T": ("Translate", c) if c != (0, 0, 0) or sc or rot else None,
+            "S": ("Scale", tuple(sc)) if sc else None, "R": ("Rotate", tuple(rot)) if rot else None}
+    return [have[k] for k in ins.get("order", "TSR") if have[k]]
 
 
 def write_ply(path, tris, normals=None, uvs=None):
@@ -464,11 +507,7 @@ def write_pbrt(dirname, name, scene, xres, yres, spp, max_depth=5, strategy="uni
                   '  Shape "plymesh" "string filename" "%s"' % ply, "ObjectEnd"]
     for ins in getattr(scene, "instance_specs", ()):
         lines.append("AttributeBegin")
-        c = ins.get("center", (0, 0, 0))
-        if tuple(c) != (0, 0, 0) or ins.get("scale"):
-            lines.append("  Translate %.9g %.9g %.9g" % tuple(c))
-        if ins.get("scale"):
-            lines.append("  Scale %.9g %.9g %.9g" % tuple(ins["scale"]))
+        lines += ["  %s %s" % (op, " ".join("%.9g" % v for v in args)) for op, args in instance_steps(ins)]
         lines += ['  ObjectInstance "obj%d"' % ins["object"], "AttributeEnd"]
     for sp in getattr(scene, "sphere_specs", ()):
         lines.append("AttributeBegin")

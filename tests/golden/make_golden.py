@@ -1,6 +1,6 @@
 """Regenerates tests/golden/* from the UNMODIFIED reference (oracle/_ref/).
 
-Run here (the container that has /root/reference):  python tests/golden/make_golden.py
+Run here (the container that has /root/reference):  python tests/golden/make_golden.py [render case ...]
 Fixtures:
   sobol_tables.bin   generator matrices dumped from core/sobolmatrices.cpp (first 256 dims)
   probe.json         camera matrices, Sobol' sample streams, camera rays, material constants
@@ -202,7 +202,14 @@ def main():
     np.save(os.path.join(HERE, "isect_rays.npy"), rays)
     np.save(os.path.join(HERE, "isect_ref.npy"), res)
 
-    for name, (nt, mats, w, h, spp, depth, strat, nl) in RENDERS.items():
+    reference_renders(RENDERS)
+    print("golden fixtures written to", HERE)
+
+
+def reference_renders(names):
+    """render_<name>.pfm of the reference for the given tests/render_cases.py RENDERS."""
+    for name in names:
+        nt, mats, w, h, spp, depth, strat, nl = RENDERS[name]
         ex = EXTRA.get(name, {})
         arr = scenes.SceneArrays(nt, materials=mats, soup_version=1, n_lights=nl, **ex.get("scene", {}))
         path = scenes.write_pbrt("/tmp/golden_render", "render_" + name, arr, w, h, spp, max_depth=depth,
@@ -210,8 +217,10 @@ def main():
         ob.run_pbrt_ref(path, threads=1 if name.startswith("filter_") else None)
         os.replace(os.path.join("/tmp/golden_render", "render_%s.pfm" % name),
                    os.path.join(HERE, "render_%s.pfm" % name))
-    print("golden fixtures written to", HERE)
 
 
 if __name__ == "__main__":
-    main()
+    if len(sys.argv) > 1:  # only the named render cases, e.g. one just added to tests/render_cases.py
+        reference_renders(sys.argv[1:])
+    else:
+        main()

@@ -32,6 +32,9 @@ RENDERS = {
     "sphere_partial": (3000, ("matte", "plastic"), 48, 40, 8, 5, "spatial", 4),
     # object instancing (TransformedPrimitive): two objects, five instances (one at the identity, one mirrored)
     "instances": (2000, ("matte", "glass", "metal", "plastic"), 48, 40, 8, 6, "spatial", None),
+    # instances under rotations about oblique axes: T S R (non-orthogonal linear part), T R S, R T S, mirrored and rotated,
+    # one at the identity -- full instance matrices for the normal transform, the error offset and the world boxes
+    "instances_affine": (2000, ("matte", "glass", "metal", "plastic"), 48, 40, 8, 6, "spatial", None),
     # MirrorMaterial (SpecularReflection + FresnelNoOp) next to glass: long specular chains
     "mirror": (3000, ("matte", "mirror", "glass", "plastic"), 40, 32, 8, 8, "spatial", None),
     # delta lights (point, spot, distant) next to the area lights: no MIS branch, Light::Power / Sample_Li per kind
@@ -74,6 +77,16 @@ EXTRA = {"lens_flip": dict(scene=dict(two_sided=True, reverse_orientation=(1, 3)
              instances=(dict(object=0, center=(0.0, 0.0, -2.4)), dict(object=0, center=(1.2, 0.8, -2.0), scale=(0.7, 1.4, 1.0)),
                         dict(object=1, center=(-1.1, -0.7, -2.2), scale=(1.0, 1.0, -1.3)), dict(object=1),
                         dict(object=0, center=(-1.3, 0.9, -1.9), scale=(1.5, 1.5, 1.5))))),
+         "instances_affine": dict(scene=dict(
+             objects=(dict(n_tris=400, seed=5, material="plastic", size=0.35), dict(n_tris=150, seed=9, material="glass", size=0.5),
+                      dict(n_tris=300, seed=13, material="metal", size=0.3)),
+             instances=(dict(object=0, center=(0.0, 0.0, -2.4), rotate=(35.0, 1.0, 2.0, -0.5)),
+                        dict(object=0, center=(1.2, 0.8, -2.0), scale=(0.7, 1.4, 1.0), rotate=(60.0, 0.3, -1.0, 0.2)),
+                        dict(object=2, center=(-1.2, 0.9, -1.9), scale=(1.5, 0.6, 1.2), rotate=(-50.0, 1.0, 1.0, 0.0), order="TRS"),
+                        dict(object=1, center=(-1.1, -0.7, -2.2), scale=(1.0, 1.0, -1.3), rotate=(120.0, -0.4, 0.7, 1.0)),
+                        dict(object=2, center=(0.9, -0.8, -2.1), scale=(1.2, 1.2, 1.2), rotate=(25.0, 0.0, 0.0, 1.0), order="RTS"),
+                        dict(object=0, center=(0.3, -1.1, -1.6), scale=(-0.8, 0.9, 0.9), rotate=(80.0, 2.0, -1.0, 1.0)),
+                        dict(object=1)))),
          "delta_lights": dict(scene=dict(delta_lights=(
              dict(kind="point", from_=(0.5, 1.5, -2.5), I=6.0),
              dict(kind="spot", from_=(-2.0, 2.0, -3.0), to=(0.0, 0.0, 0.0), I=(30.0, 24.0, 18.0), coneangle=25.0, conedelta=8.0),

@@ -117,15 +117,17 @@ def test_dropin_binary_matches_reference(scenes, tmp_path):
     got = scenes.read_pfm(os.path.join(str(tmp_path), "render_filter_gaussian.pfm"))
     ref = scenes.read_pfm(os.path.join(GOLDEN, "render_filter_gaussian.pfm"))
     assert np.array_equal(bits(got), bits(ref)), "drop-in render (Gaussian pixel filter) differs from the reference"
-    # object instancing: ObjectBegin / ObjectInstance blocks become TransformedPrimitives over per-object BVHAccels
-    nt, mats, w, h, spp, depth, strat, nl = RENDERS["instances"]
-    arr = scenes.SceneArrays(nt, materials=mats, soup_version=1, n_lights=nl, **EXTRA["instances"]["scene"])
-    path = scenes.write_pbrt(str(tmp_path), "render_instances", arr, w, h, spp, max_depth=depth, strategy=strat)
-    r = subprocess.run([PLUGIN, "--quiet", os.path.basename(path)], cwd=str(tmp_path), capture_output=True, text=True)
-    assert r.returncode == 0, r.stdout + r.stderr
-    got = scenes.read_pfm(os.path.join(str(tmp_path), "render_instances.pfm"))
-    ref = scenes.read_pfm(os.path.join(GOLDEN, "render_instances.pfm"))
-    assert np.array_equal(bits(got), bits(ref)), "drop-in render (object instances) differs from the reference"
+    # object instancing: ObjectBegin / ObjectInstance blocks become TransformedPrimitives over per-object BVHAccels; the
+    # rotated instances carry the matrices of pbrt's own Rotate
+    for name in ("instances", "instances_affine"):
+        nt, mats, w, h, spp, depth, strat, nl = RENDERS[name]
+        arr = scenes.SceneArrays(nt, materials=mats, soup_version=1, n_lights=nl, **EXTRA[name]["scene"])
+        path = scenes.write_pbrt(str(tmp_path), "render_" + name, arr, w, h, spp, max_depth=depth, strategy=strat)
+        r = subprocess.run([PLUGIN, "--quiet", os.path.basename(path)], cwd=str(tmp_path), capture_output=True, text=True)
+        assert r.returncode == 0, r.stdout + r.stderr
+        got = scenes.read_pfm(os.path.join(str(tmp_path), "render_%s.pfm" % name))
+        ref = scenes.read_pfm(os.path.join(GOLDEN, "render_%s.pfm" % name))
+        assert np.array_equal(bits(got), bits(ref)), "drop-in render (object instances, %s) differs from the reference" % name
     # delta lights and the mirror material, parsed by the reference's own factories
     for name in ("delta_lights", "mirror"):
         nt, mats, w, h, spp, depth, strat, nl = RENDERS[name]

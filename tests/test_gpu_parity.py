@@ -159,7 +159,12 @@ def test_trace_instances_vs_oracle(pkg, abi, scenes, ob, ctx):
     # 5 instances are tested one by one; 40 go through the tree over their leaf boxes
     lattice = tuple(dict(object=k % 2, center=(-0.9 + 0.45 * (k % 5), -0.7 + 0.45 * ((k // 5) % 4), -0.5 + 0.9 * (k // 20)),
                          scale=(0.5, 0.5, -0.5 if k % 3 == 0 else 0.5)) for k in range(40))
-    for n_tris, instances in ((0, instances), (3000, instances), (3000, lattice)):
+    # the same lattice under rotations about oblique axes in three step orders, every third one mirrored: full 3x3 linear
+    # parts (non-orthogonal ones for T S R) in the ray transform, its error offset and the instances' world boxes
+    affine = tuple(dict(ins, scale=(0.5, 0.4 + 0.05 * (k % 4), ins["scale"][2]), rotate=((17.0 + 23.0 * k) % 360, 1.0, k % 7 - 3.0,
+                                                                                           0.5 + k % 3), order=("TSR", "TRS", "RTS")[k % 3])
+                   for k, ins in enumerate(lattice))
+    for n_tris, instances in ((0, instances), (3000, instances), (3000, lattice), (3000, affine)):
         arr = scenes.SceneArrays(n_tris, materials=("matte",), soup_version=1, seed=21, n_lights=0, objects=objects,
                                  instances=instances)
         scene = pkg.Scene(ctx, arr.desc(), keepalive=arr)

@@ -12,9 +12,9 @@ import pytest
 
 import test_gpu_parity as G
 import test_zz_spectral_gpu as GS
+import test_zz_sweeps_gpu as GW
 import test_zz_volpath_gpu as GV
-from conftest import GOLDEN, bits
-from render_cases import EXTRA, RENDERS
+from render_cases import RENDERS
 
 
 @pytest.fixture(scope="module")
@@ -131,6 +131,19 @@ def test_fullsize_checks_at_a_small_film(hostcheck, abi, scenes, ob, hctx, monke
     F.test_fullsize_spectral_cfg5_shape(hostcheck, abi, scenes, ob, hctx, monkeypatch, film=(160, 90, 8), n_tris=2000, batch_tiles=7)
     F.test_fullsize_volpath_cfg2fog_shape(hostcheck, abi, scenes, ob, hctx, monkeypatch, film=(160, 90, 16), n_tris=20000,
                                           batch_tiles=7)
+
+
+def test_instance_lattice_checks_at_a_small_size(hostcheck, abi, scenes, ob, hctx, monkeypatch, tmp_path):
+    """The benchmark-lattice tests (tests/test_zz_instances_gpu.py) with small objects, a 5000-triangle soup and 4000 rays
+    per family.  The check build has no k_trace2: both arms of the comparison are k_spheres' InstanceWalk here, so this
+    checks the tests' own logic (the child process, the ray families, the near-tie rule, the films) and the oracle side,
+    not the two-level kernel."""
+    import test_zz_instances_gpu as I
+    I.test_lattices_are_the_benchmarks()
+    I.check_lattice(hostcheck, abi, scenes, ob, hctx, monkeypatch, tmp_path / "cfg5", "cfg5", n_soup=5000, n_tris=2000, n_rays=4000)
+    I.check_lattice(hostcheck, abi, scenes, ob, hctx, monkeypatch, tmp_path / "cfg5s", "cfg5s", n_soup=5000, n_tris=5000, n_rays=4000)
+    for spectral in (False, True):
+        I.test_separated_lattice_renders_vs_oracle(hostcheck, abi, scenes, ob, hctx, monkeypatch, spectral, n_soup=5000, n_tris=2000)
 
 
 def test_device_bvh_builder_is_refused(hostcheck, abi, scenes, hctx):
@@ -362,13 +375,7 @@ def test_bad_render_descriptors_are_refused(hostcheck, abi, scenes, hctx):
 
 
 def test_new_paths_in_several_batches(hostcheck, abi, scenes, ob, hctx, monkeypatch):
-    """The 60-bin state arrays are planar [bin][capacity] and the medium pass shares the per-slot direct-lighting records
-    with the shading kernels: render with a capacity of three tiles per batch (many batches) and compare as before."""
-    monkeypatch.setenv("B200PT_BATCH_PATHS", str(256 * 8 * 3))
-    GS.test_spectral_render_and_counters_vs_oracle(hostcheck, abi, scenes, ob, hctx, ("matte", "glass", "metal", "plastic"), 8, "power", None)
-    GV.test_volpath_render_vs_oracle(hostcheck, abi, scenes, ob, hctx, ("matte", "plastic"), 12, "uniform",
-                                     dict(sigma_a=(0.2, 0.2, 0.2), sigma_s=(1.5, 1.2, 0.9), g=-0.5), {})
-    GS.test_spectral_volpath_render_vs_sampled_spectrum_reference(hostcheck, abi, scenes, ob, hctx, "spectral_volpath_fog", "volpath_fog")
+    GW.test_new_paths_in_several_batches(hostcheck, abi, scenes, ob, hctx, monkeypatch)
 
 
 def test_dropin_refuses_media_it_does_not_support(hc_plugins, scenes, tmp_path):
@@ -410,86 +417,14 @@ def test_feature_combinations_vs_oracle(hostcheck, abi, scenes, ob, hctx, combo)
 
 @pytest.mark.parametrize("spectral", [False, True])
 def test_sample_clamp_crop_and_scale_vs_oracle(hostcheck, abi, scenes, ob, hctx, spectral):
-    """Film options that look at the sample's luminance -- "maxsampleluminance" (film.h:124-125, y() of the sample: the
-    60-bin y() rounds differently from ToXYZ's Y) --, a crop window and the film scale, box and Gaussian filter."""
-    import json
-    tables = json.load(open(os.path.join(GOLDEN, "spectral_tables.json"))) if spectral else None
-    arr = scenes.SceneArrays(3000, materials=("matte", "glass", "metal", "plastic"), soup_version=1)
-    if spectral:
-        arr.attach_spectral(tables)
-    scene = hostcheck.Scene(hctx, arr.desc(), keepalive=arr)
-    o = ob.Oracle(abi, arr, spectral_tables=tables)
-    for kw in (dict(max_sample_luminance=3.0, film_scale=0.5, crop_window=(0.1, 0.9, 0.2, 0.8)),
-               dict(max_sample_luminance=1.5, pixel_filter="gaussian")):
-        setup = scenes.RenderSetup(48, 32, 8, max_depth=5, strategy=abi.LIGHTS_UNIFORM, **kw)
-        film, _ = o.render(setup, threads=4)
-        r = hostcheck.Render(scene, setup)
-        r.render_tiles()
-        assert np.array_equal(bits(r.read_raw()), bits(film))
-        assert np.array_equal(bits(r.read_rgb()), bits(o.film_rgb(setup, film)))
-        clamped = float(np.nan_to_num(r.read_rgb()).max())
-        r.close()
-        r2 = hostcheck.Render(scene, scenes.RenderSetup(48, 32, 8, max_depth=5, strategy=abi.LIGHTS_UNIFORM,
-                                                         **{k: v for k, v in kw.items() if k != "max_sample_luminance"}))
-        r2.render_tiles()
-        assert float(np.nan_to_num(r2.read_rgb()).max()) > clamped  # the clamp really was active
-        r2.close()
-    scene.close()
-    o.close()
+    GW.test_sample_clamp_crop_and_scale_vs_oracle(hostcheck, abi, scenes, ob, hctx, spectral)
 
 
 @pytest.mark.parametrize("name", sorted(RENDERS))
 def test_every_golden_scene_under_sampled_spectrum_vs_oracle(hostcheck, abi, scenes, ob, hctx, name):
-    """Every scene of the RGB golden set again with a SampledSpectrum host (where the fixtures hold its spectra): the 60-bin
-    kernels against the 60-bin oracle (itself pinned against the SampledSpectrum reference on seven of these scenes)."""
-    import json
-    tables = json.load(open(os.path.join(GOLDEN, "spectral_tables.json")))
-    nt, mats, w, h, spp, depth, strat, nl = RENDERS[name]
-    ex = EXTRA.get(name, {})
-    arr = scenes.SceneArrays(nt, materials=mats, soup_version=1, n_lights=nl, **ex.get("scene", {}))
-    try:
-        arr.attach_spectral(tables)
-    except KeyError as e:
-        pytest.skip("no 60-bin fixture: %s" % e)
-    setup = scenes.RenderSetup(w, h, spp, max_depth=depth, strategy=getattr(abi, GV.STRATEGY[strat]), **ex.get("camera", {}))
-    o = ob.Oracle(abi, arr, spectral_tables=tables)
-    film, ostats = o.render(setup, threads=4)
-    scene = hostcheck.Scene(hctx, arr.desc(), keepalive=arr)
-    r = hostcheck.Render(scene, setup)
-    r.render_tiles()
-    assert np.array_equal(bits(r.read_raw()), bits(film))
-    st = r.stats()
-    # (MIS rays towards a sphere light that miss the sphere are not traced on the device -- Sphere::Pdf is non-zero for
-    # them, the reference traces them in vain --, so "regular" rays are only bounded)
-    assert st["camera_rays"] == ostats["camera_rays"] and st["shadow_rays"] == ostats["shadow_rays"]
-    assert st["regular_rays"] <= ostats["regular_rays"]
-    r.close()
-    scene.close()
-    o.close()
+    GW.test_every_golden_scene_under_sampled_spectrum_vs_oracle(hostcheck, abi, scenes, ob, hctx, name)
 
 
 @pytest.mark.parametrize("name", sorted(RENDERS))
 def test_every_golden_scene_in_fog_under_volpath_vs_oracle(hostcheck, abi, scenes, ob, hctx, name):
-    """Every scene of the golden set again with `Integrator "volpath"` inside a homogeneous medium: the medium pass meets
-    every shape, light, sampler, filter and camera option of the set; device (check build) against the oracle's VolPathLi
-    (itself pinned against the reference's volpath on four of these scenes)."""
-    fog = dict(sigma_a=(0.04, 0.06, 0.08), sigma_s=(0.25, 0.2, 0.3), g=0.35)
-    nt, mats, w, h, spp, depth, strat, nl = RENDERS[name]
-    ex = EXTRA.get(name, {})
-    arr = scenes.SceneArrays(nt, materials=mats, soup_version=1, n_lights=nl, **ex.get("scene", {}))
-    setup = scenes.RenderSetup(w, h, spp, max_depth=depth, strategy=getattr(abi, GV.STRATEGY[strat]), integrator="volpath",
-                               medium=fog, **ex.get("camera", {}))
-    o = ob.Oracle(abi, arr)
-    ob.set_volpath(o.lib, True, fog)
-    try:
-        film, ostats = o.render(setup, threads=4)
-    finally:
-        ob.set_volpath(o.lib, False)
-    scene = hostcheck.Scene(hctx, arr.desc(), keepalive=arr)
-    r = hostcheck.Render(scene, setup)
-    r.render_tiles()
-    assert np.array_equal(bits(r.read_raw()), bits(film))
-    assert r.stats()["camera_rays"] == ostats["camera_rays"]
-    r.close()
-    scene.close()
-    o.close()
+    GW.test_every_golden_scene_in_fog_under_volpath_vs_oracle(hostcheck, abi, scenes, ob, hctx, name)
