@@ -87,7 +87,11 @@ typedef struct b200pt_material {
  * (lights/point.cpp:43-56), SpotLight (lights/spot.cpp:42-76) and DistantLight
  * (lights/distant.cpp:43-66): no geometry, no BSDF-sampling branch in
  * EstimateDirect (integrator.cpp:166). */
-enum { B200PT_LIGHT_AREA = 0, B200PT_LIGHT_POINT = 1, B200PT_LIGHT_SPOT = 2, B200PT_LIGHT_DISTANT = 3 };
+enum { B200PT_LIGHT_AREA = 0, B200PT_LIGHT_POINT = 1, B200PT_LIGHT_SPOT = 2, B200PT_LIGHT_DISTANT = 3,
+       /* InfiniteAreaLight (lights/infinite.cpp:43-132), PathIntegrator on RGBSpectrum hosts only: world_to_light and
+        * world_radius (0 = computed from the scene bounds) are used here, the map and its sampling tables are set with
+        * b200pt_scene_set_infinite_light before b200pt_render_create */
+       B200PT_LIGHT_INFINITE = 4 };
 typedef struct b200pt_area_light {
     int32_t triangle;    /* area light: index into the triangle arrays                */
     float lemit[3];      /* area: Lemit; point / spot: I; distant: L (all already multiplied by "scale") */
@@ -353,6 +357,27 @@ int b200pt_scene_upload(b200pt_scene *scene, uint64_t *bytes);
 /* bytes of device memory held by nodes / triangles, node count */
 int b200pt_scene_info(const b200pt_scene *scene, uint64_t *node_bytes, uint64_t *tri_bytes,
                       uint64_t *n_nodes);
+
+/* ---- infinite area lights: what InfiniteAreaLight (lights/infinite.cpp:43-84) holds, copied, never recomputed.
+ * Le and Sample_Li look the map up with width 0, which is the bilinear lookup of pyramid level 0 with Repeat wrap
+ * (MIPMap::Lookup / triangle, mipmap.h:245-273): level 0 is all the device needs.  The Distribution2D
+ * (sampling.h:124-141) is passed as the host built it from the trilinear lookups of the whole pyramid. */
+typedef struct b200pt_infinite_light {
+    int32_t width, height;          /* Lmap->pyramid[0]: uSize(), vSize() (a power of two each after resampling) */
+    const float *texels;            /* [height][width][3] RGB texels of level 0                                  */
+    float light_to_world[16];       /* Light::LightToWorld.m (row-major)                                         */
+    int32_t nu, nv;                 /* Distribution2D: nv conditional rows of nu entries each                    */
+    const float *cond_func;         /* [nv][nu]   pConditionalV[v]->func                                         */
+    const float *cond_cdf;          /* [nv][nu+1] pConditionalV[v]->cdf                                          */
+    const float *cond_func_int;     /* [nv]       pConditionalV[v]->funcInt                                      */
+    const float *marg_func;         /* [nv]       pMarginal->func                                                */
+    const float *marg_cdf;          /* [nv+1]     pMarginal->cdf                                                 */
+    float marg_func_int;            /* pMarginal->funcInt                                                        */
+    float power_rgb[3];             /* Lmap->Lookup(Point2f(.5f, .5f), .5f), for Power() (infinite.cpp:86-90)    */
+} b200pt_infinite_light;
+/* Sets the map and tables of light `light` (kind B200PT_LIGHT_INFINITE) of the scene; the library copies them.  Call it
+ * between b200pt_scene_create and b200pt_render_create, once per infinite light. */
+int b200pt_scene_set_infinite_light(b200pt_scene *scene, int32_t light, const b200pt_infinite_light *desc);
 
 /* ---- kernel-level entry points (parity tests, traversal benchmarks) -------
  * Replace Scene::Intersect / Scene::IntersectP (core/scene.cpp:45-55) on

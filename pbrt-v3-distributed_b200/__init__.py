@@ -41,6 +41,7 @@ _SIGNATURES = {
     "b200pt_scene_destroy": (None, [_vp]),
     "b200pt_scene_upload": (C.c_int, [_vp, C.POINTER(_u64)]),
     "b200pt_scene_info": (C.c_int, [_vp, C.POINTER(_u64), C.POINTER(_u64), C.POINTER(_u64)]),
+    "b200pt_scene_set_infinite_light": (C.c_int, [_vp, _i32, C.POINTER(abi.InfiniteLight)]),
     "b200pt_trace_closest": (C.c_int, [_vp, _vp, _vp, _i64]),
     "b200pt_trace_any": (C.c_int, [_vp, _vp, _vp, _i64]),
     "b200pt_trace_closest_dev": (C.c_int, [_vp, _u64, _u64, _i64]),
@@ -170,6 +171,22 @@ class Scene:
         a, b, c = _u64(), _u64(), _u64()
         _check(lib.b200pt_scene_info(self.h, C.byref(a), C.byref(b), C.byref(c)))
         return {"node_bytes": a.value, "tri_bytes": b.value, "n_nodes": c.value}
+
+    def set_infinite_light(self, light, tables):
+        """b200pt_scene_set_infinite_light: `tables` is a dict of the host's InfiniteAreaLight data -- texels [h][w][3],
+        light_to_world (16), cond_func [nv][nu], cond_cdf [nv][nu+1], cond_func_int [nv], marg_func [nv],
+        marg_cdf [nv+1], marg_func_int, power_rgb (3).  The library copies them."""
+        f32 = lambda k: np.ascontiguousarray(tables[k], dtype=np.float32)
+        arrs = {k: f32(k) for k in ("texels", "cond_func", "cond_cdf", "cond_func_int", "marg_func", "marg_cdf")}
+        rec = abi.InfiniteLight()
+        rec.height, rec.width = arrs["texels"].shape[:2]
+        rec.nv, rec.nu = arrs["cond_func"].shape
+        for k, a in arrs.items():
+            setattr(rec, k, a.ctypes.data)
+        rec.light_to_world[:] = [float(v) for v in f32("light_to_world").reshape(-1)]
+        rec.marg_func_int = float(np.float32(tables["marg_func_int"]))
+        rec.power_rgb[:] = [float(v) for v in f32("power_rgb")]
+        _check(lib.b200pt_scene_set_infinite_light(self.h, int(light), C.byref(rec)))
 
     def trace_closest(self, rays):
         rays = np.ascontiguousarray(rays, dtype=abi.RAY_DTYPE)

@@ -64,7 +64,15 @@ class FilmDesc(C.Structure):
 
 SAMPLER_SOBOL, SAMPLER_HALTON = 0, 1
 SPECTRUM_SAMPLES, MATERIAL_SPECTRA = 60, 5  # B200PT_SPECTRUM_SAMPLES, B200PT_MATERIAL_SPECTRA
-LIGHT_AREA, LIGHT_POINT, LIGHT_SPOT, LIGHT_DISTANT = 0, 1, 2, 3
+LIGHT_AREA, LIGHT_POINT, LIGHT_SPOT, LIGHT_DISTANT, LIGHT_INFINITE = 0, 1, 2, 3, 4
+
+
+class InfiniteLight(C.Structure):
+    """b200pt_infinite_light: level 0 of an InfiniteAreaLight's map and its Distribution2D tables."""
+    _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("texels", C.c_void_p), ("light_to_world", C.c_float * 16),
+                ("nu", C.c_int32), ("nv", C.c_int32), ("cond_func", C.c_void_p), ("cond_cdf", C.c_void_p),
+                ("cond_func_int", C.c_void_p), ("marg_func", C.c_void_p), ("marg_cdf", C.c_void_p),
+                ("marg_func_int", C.c_float), ("power_rgb", C.c_float * 3)]
 
 
 class SamplerDesc(C.Structure):

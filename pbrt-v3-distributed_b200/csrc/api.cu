@@ -83,6 +83,12 @@ struct b200pt_scene {
     int nspec = 0;
     std::vector<float> material_spectra, light_spectra, cie_xyz;
     float *d_material_spectra = nullptr;
+    // infinite area lights (b200pt_scene_set_infinite_light), by light index: the device tables (pointers into
+    // d_infinite_tables[light]) and Power()'s RGB; infinite_set[light] == 0: no map set yet
+    std::vector<DevInfinite> infinite;
+    std::vector<float> infinite_power;  // [n_lights][3]
+    std::vector<char> infinite_set;
+    std::vector<void *> d_infinite_tables;
 };
 
 struct TimedLaunch {
@@ -261,7 +267,7 @@ int b200pt_scene_create(b200pt_ctx *ctx, const b200pt_scene_desc *d, b200pt_scen
     }
     for (int i = 0; i < d->n_lights; ++i) {
         const int kind = d->lights[i].kind;
-        if (kind < B200PT_LIGHT_AREA || kind > B200PT_LIGHT_DISTANT)
+        if (kind < B200PT_LIGHT_AREA || kind > B200PT_LIGHT_INFINITE)
             return b200pt_fail(B200PT_ERR_INVALID, "scene_create: light %d has unknown kind %d", i, kind);
         if (kind != B200PT_LIGHT_AREA) continue;  // delta lights have no geometry
         const int sph = d->lights[i].sphere;
@@ -696,10 +702,67 @@ void b200pt_scene_destroy(b200pt_scene *s) {
     cudaFree(s->d_spheres);
     cudaFree(s->d_instances);
     cudaFree(s->d_work);
+    for (void *p : s->d_infinite_tables) cudaFree(p);
     cudaFreeHost(s->h_nodes);
     cudaFreeHost(s->h_tri_base);
     cudaFreeHost(s->h_tris);
     delete s;
+}
+
+int b200pt_scene_set_infinite_light(b200pt_scene *s, int32_t light, const b200pt_infinite_light *d) {
+    if (!s || !d) return b200pt_fail(B200PT_ERR_INVALID, "scene_set_infinite_light: NULL argument");
+    if (light < 0 || light >= (int32_t)s->lights.size() || s->lights[light].kind != B200PT_LIGHT_INFINITE)
+        return b200pt_fail(B200PT_ERR_INVALID, "scene_set_infinite_light: light %d is not an infinite light", light);
+    if (d->width <= 0 || d->height <= 0 || d->nu <= 0 || d->nv <= 0 || (int64_t)d->width * d->height > (1ll << 28) ||
+        (int64_t)d->nu * d->nv > (1ll << 28))
+        return b200pt_fail(B200PT_ERR_INVALID, "scene_set_infinite_light: bad map (%d x %d) or distribution (%d x %d) size", d->width,
+                           d->height, d->nu, d->nv);
+    if (!d->texels || !d->cond_func || !d->cond_cdf || !d->cond_func_int || !d->marg_func || !d->marg_cdf)
+        return b200pt_fail(B200PT_ERR_INVALID, "scene_set_infinite_light: a table is NULL");
+    CUDA_TRY(cudaSetDevice(s->ctx->device));
+    const size_t nt = (size_t)d->width * d->height, nu = (size_t)d->nu, nv = (size_t)d->nv;
+    // one allocation: texels (float4), then cond_func, cond_cdf, cond_func_int, marg_func, marg_cdf
+    std::vector<float> h(4 * nt + nv * nu + nv * (nu + 1) + nv + nv + (nv + 1));
+    for (size_t i = 0; i < nt; ++i)
+        for (int c = 0; c < 3; ++c) h[4 * i + c] = d->texels[3 * i + c];
+    const size_t o_cf = 4 * nt, o_cc = o_cf + nv * nu, o_ci = o_cc + nv * (nu + 1), o_mf = o_ci + nv, o_mc = o_mf + nv;
+    memcpy(h.data() + o_cf, d->cond_func, nv * nu * sizeof(float));
+    memcpy(h.data() + o_cc, d->cond_cdf, nv * (nu + 1) * sizeof(float));
+    memcpy(h.data() + o_ci, d->cond_func_int, nv * sizeof(float));
+    memcpy(h.data() + o_mf, d->marg_func, nv * sizeof(float));
+    memcpy(h.data() + o_mc, d->marg_cdf, (nv + 1) * sizeof(float));
+    float *dp = nullptr;
+    if (cudaMalloc(&dp, h.size() * sizeof(float)) != cudaSuccess)
+        return b200pt_fail(B200PT_ERR_OOM, "scene_set_infinite_light: cudaMalloc of %zu bytes failed", h.size() * sizeof(float));
+    if (cudaMemcpy(dp, h.data(), h.size() * sizeof(float), cudaMemcpyHostToDevice) != cudaSuccess) {
+        cudaFree(dp);
+        return b200pt_fail(B200PT_ERR_CUDA, "scene_set_infinite_light: upload failed");
+    }
+    const size_t nl = s->lights.size();
+    s->infinite.resize(nl);
+    s->infinite_power.resize(3 * nl);
+    s->infinite_set.resize(nl, 0);
+    s->d_infinite_tables.resize(nl, nullptr);
+    cudaFree(s->d_infinite_tables[light]);
+    s->d_infinite_tables[light] = dp;
+    DevInfinite &L = s->infinite[light];
+    memset(&L, 0, sizeof(L));
+    L.w = d->width;
+    L.h = d->height;
+    L.texels = reinterpret_cast<const float4 *>(dp);
+    memcpy(L.light_to_world, d->light_to_world, sizeof(L.light_to_world));
+    memcpy(L.world_to_light, s->lights[light].world_to_light, sizeof(L.world_to_light));
+    L.nu = d->nu;
+    L.nv = d->nv;
+    L.cond_func = dp + o_cf;
+    L.cond_cdf = dp + o_cc;
+    L.cond_func_int = dp + o_ci;
+    L.marg_func = dp + o_mf;
+    L.marg_cdf = dp + o_mc;
+    L.marg_func_int = d->marg_func_int;
+    memcpy(&s->infinite_power[3 * (size_t)light], d->power_rgb, 3 * sizeof(float));
+    s->infinite_set[light] = 1;
+    return B200PT_OK;
 }
 
 int b200pt_scene_info(const b200pt_scene *s, uint64_t *node_bytes, uint64_t *tri_bytes, uint64_t *n_nodes) {
@@ -910,6 +973,17 @@ int b200pt_render_create(b200pt_scene *scene, const b200pt_camera_desc *cam, con
     if (integ->light_strategy != B200PT_LIGHTS_UNIFORM && integ->light_strategy != B200PT_LIGHTS_POWER &&
         integ->light_strategy != B200PT_LIGHTS_SPATIAL)
         return b200pt_fail(B200PT_ERR_INVALID, "render_create: unsupported light sample strategy");
+    for (size_t i = 0; i < scene->lights.size(); ++i) {
+        if (scene->lights[i].kind != B200PT_LIGHT_INFINITE) continue;
+        // Spectrum(RGBSpectrum, Illuminant) is a per-lookup FromRGB on SampledSpectrum hosts (infinite.cpp:95), which the
+        // device does not restate; VolPathIntegrator's escaped rays and transmittance are not built for these lights
+        if (scene->nspec)
+            return b200pt_fail(B200PT_ERR_INVALID, "render_create: infinite lights are not supported for SampledSpectrum hosts");
+        if (integ->volumetric)
+            return b200pt_fail(B200PT_ERR_INVALID, "render_create: infinite lights are not supported with the volumetric integrator");
+        if (i >= scene->infinite_set.size() || !scene->infinite_set[i])
+            return b200pt_fail(B200PT_ERR_INVALID, "render_create: infinite light %zu has no map (b200pt_scene_set_infinite_light)", i);
+    }
     const int sbw = smp->sample_bounds[2] - smp->sample_bounds[0], sbh = smp->sample_bounds[3] - smp->sample_bounds[1];
     if (sbw <= 0 || sbh <= 0) return b200pt_fail(B200PT_ERR_INVALID, "render_create: empty sample bounds");
     const int cw = film->cropped_bounds[2] - film->cropped_bounds[0], chh = film->cropped_bounds[3] - film->cropped_bounds[1];
@@ -1043,11 +1117,28 @@ int b200pt_render_create(b200pt_scene *scene, const b200pt_camera_desc *cam, con
         world_radius = inside ? len(c - mk(hi[0], hi[1], hi[2])) : 0.f;
     }
     bool has_delta = false;
+    std::vector<DevInfinite> infinite;  // Scene::infiniteLights order
     for (int i = 0; i < nl; ++i) {
         const b200pt_area_light &sl = scene->lights[i];
         memset(&dl[i], 0, sizeof(DevLight));
         memcpy(dl[i].lemit, sl.lemit, sizeof(float) * 3);
         dl[i].kind = sl.kind;
+        if (sl.kind == B200PT_LIGHT_INFINITE) {
+            // InfiniteAreaLight::Preprocess (infinite.h:57-59): the same bounding sphere as the distant light's
+            const float wr = sl.world_radius != 0.f ? sl.world_radius : world_radius;
+            dl[i].tri = B200PT_MISS;  // the MIS ray reaches this light when it hits nothing (k_resolve)
+            dl[i].two_sided = (int)infinite.size();
+            infinite.push_back(scene->infinite[i]);
+            infinite.back().two_world_radius = 2 * wr;
+            if (integ->light_strategy == B200PT_LIGHTS_POWER && nl != 1) {
+                // InfiniteAreaLight::Power() (infinite.cpp:86-90): Pi * worldRadius * worldRadius * rgb, then y()
+                const float k = PT_PI * wr * wr;
+                const float *rgbp_ = &scene->infinite_power[3 * (size_t)i];
+                std::vector<float> p = {k * rgbp_[0], k * rgbp_[1], k * rgbp_[2]};
+                func[i] = host_spectrum_y(scene, p);
+            }
+            continue;
+        }
         if (sl.kind != B200PT_LIGHT_AREA) {
             has_delta = true;
             dl[i].tri = B200PT_MISS;
@@ -1134,6 +1225,7 @@ int b200pt_render_create(b200pt_scene *scene, const b200pt_camera_desc *cam, con
     cudaError_t e = cudaSuccess;
     uint32_t *mat32 = nullptr, *sobol_table = nullptr;
     DevLight *d_lights = nullptr;
+    DevInfinite *d_infinite = nullptr;
     float *d_cdf = nullptr, *d_func = nullptr;
 #define ALLOC(ptr, count) \
     if (e == cudaSuccess) e = dev_alloc(r, &(ptr), (count))
@@ -1148,6 +1240,7 @@ int b200pt_render_create(b200pt_scene *scene, const b200pt_camera_desc *cam, con
         ALLOC(sobol_table, (size_t)smp->n_dimensions * 5 * 256);
     }
     ALLOC(d_lights, (size_t)nl);
+    if (!infinite.empty()) ALLOC(d_infinite, infinite.size());
     ALLOC(d_cdf, (size_t)nl + 1);
     ALLOC(d_func, (size_t)std::max(nl, 1));
     ALLOC(H.sp_func, (size_t)nvox * nl);
@@ -1245,6 +1338,8 @@ int b200pt_render_create(b200pt_scene *scene, const b200pt_camera_desc *cam, con
     H.sphere_med = d_sphere_med;
     H.dim_overflows = H.stats + 8;
     H.has_delta_lights = has_delta ? 1 : 0;
+    H.infinite = d_infinite;
+    H.n_infinite = (int)infinite.size();
     H.light_cdf = d_cdf;
     H.light_func = d_func;
     cudaStream_t st = ctx->stream;
@@ -1261,6 +1356,10 @@ int b200pt_render_create(b200pt_scene *scene, const b200pt_camera_desc *cam, con
         launch_sobol_table(mat32, sobol_table, smp->n_dimensions, st);
     }
     if (nl) CUDA_TRY(cudaMemcpyAsync(d_lights, dl.data(), nl * sizeof(DevLight), cudaMemcpyHostToDevice, st));
+    if (!infinite.empty()) {
+        CUDA_TRY(cudaMemcpyAsync(d_infinite, infinite.data(), infinite.size() * sizeof(DevInfinite), cudaMemcpyHostToDevice, st));
+        CUDA_TRY(cudaStreamSynchronize(st));  // `infinite` is a local
+    }
     if (scene->nspec) {
         if (b200pt_s60::render_dev_size() != sizeof(RenderDev)) {
             return b200pt_fail(B200PT_ERR_INVALID, "render_create: the SampledSpectrum kernels were built with another RenderDev layout");
@@ -1469,7 +1568,14 @@ int b200pt_render_tiles(b200pt_render *r, const int32_t *tiles, int64_t n_tiles)
         const bool tl = two_level(r->scene) && !r->instrumented;  // instances inside the traversal kernel
         const bool has_spheres = H.scene.n_spheres > 0 || (H.scene.n_instances > 0 && !tl);  // "extra shapes" pass needed
         const bool full_shade = has_spheres || H.scene.n_instances > 0 || H.has_delta_lights || H.scene.tri_n != nullptr ||
-                                H.scene.tri_uv != nullptr || H.volpath;
+                                H.scene.tri_uv != nullptr || H.volpath || H.n_infinite > 0;
+        // escaped path rays of bounce b (scenes with infinite lights, RGB build only): after resolve(b - 1), before shade(b + 1)
+        // rewrites the bounce's path queue
+        auto escape = [&](int b) {
+            if (H.n_infinite == 0) return;
+            LaunchTimer lt(r, st, 2);
+            launch_escape(r->d_dev, b, H.work + (size_t)b * W_PER_BOUNCE + W_ESCAPE, r->grid_shade, st);
+        };
         // traversal of one ray queue: the plain kernel, or the two-level one when the scene has instances
         auto trace = [&](TraceArgs &a, bool any_hit, bool classify, cudaStream_t s_) {
 #ifndef B200PT_HOST_EMU
@@ -1629,6 +1735,7 @@ int b200pt_render_tiles(b200pt_render *r, const int32_t *tiles, int64_t n_tiles)
             intersect(a, false, false, has_spheres, wk + W_SPHERES_MIS, st2);
         };
         trace_path(0);
+        escape(0);
         for (int b = 0; b <= maxDepth; ++b) {
             uint32_t *wk = H.work + (size_t)b * W_PER_BOUNCE;
             for (int m = 0; m < 4; ++m)
@@ -1644,6 +1751,7 @@ int b200pt_render_tiles(b200pt_render *r, const int32_t *tiles, int64_t n_tiles)
                     LAUNCH_SPEC(launch_resolve, dev, b, wk + W_RESOLVE, r->grid_shade, st);
                 }
                 trace_path(b + 1);
+                escape(b + 1);
             } else if (b < maxDepth) {  // no direct lighting is estimated at the last vertex (path.cpp:104)
                 if (overlap) {
                     CUDA_TRY(cudaEventRecord(ctx->ev_fork, st));
@@ -1653,8 +1761,11 @@ int b200pt_render_tiles(b200pt_render *r, const int32_t *tiles, int64_t n_tiles)
                 if (overlap) CUDA_TRY(cudaEventRecord(ctx->ev_join, st2));
                 trace_path(b + 1);
                 if (overlap) CUDA_TRY(cudaStreamWaitEvent(st, ctx->ev_join, 0));
-                LaunchTimer lt(r, st, 2);
-                LAUNCH_SPEC(launch_resolve, dev, b, wk + W_RESOLVE, r->grid_shade, st);
+                {
+                    LaunchTimer lt(r, st, 2);
+                    LAUNCH_SPEC(launch_resolve, dev, b, wk + W_RESOLVE, r->grid_shade, st);
+                }
+                escape(b + 1);
             }
         }
         {

@@ -1078,6 +1078,80 @@ __device__ __forceinline__ DeltaLight delta_of(const DevLight &l, const Spec &in
     return d;
 }
 
+#if B200PT_NSPEC == 3
+// ---- InfiniteAreaLight (lights/infinite.cpp:92-132) over the host's level-0 texels and Distribution2D tables
+#define PT_INV_PI ((float)0.31830988618379067154)
+#define PT_INV_2PI ((float)0.15915494309189533577)
+// MIPMap::triangle(0, st) (mipmap.h:262-273): bilinear, Repeat wrap (Mod, pbrt.h), the weights formed first
+__device__ __forceinline__ Spec infinite_lookup(const DevInfinite &L, float st0, float st1) {
+    const float s = st0 * L.w - 0.5f, t = st1 * L.h - 0.5f;
+    const int s0 = (int)floorf(s), t0 = (int)floorf(t);
+    const float ds = s - s0, dt = t - t0;
+    auto mod = [](int a, int b) {
+        const int r = a - (a / b) * b;
+        return r < 0 ? r + b : r;
+    };
+    auto texel = [&](int si, int ti) {
+        const float4 v = L.texels[(size_t)mod(ti, L.h) * L.w + mod(si, L.w)];
+        return rgb(v.x, v.y, v.z);
+    };
+    return (1 - ds) * (1 - dt) * texel(s0, t0) + (1 - ds) * dt * texel(s0, t0 + 1) + ds * (1 - dt) * texel(s0 + 1, t0) +
+           ds * dt * texel(s0 + 1, t0 + 1);
+}
+// SphericalPhi (geometry.h:1478-1481)
+__device__ __forceinline__ float spherical_phi(const V3 &v) {
+    const float p = pt_atan2f(v.y, v.x);
+    return (p < 0) ? (p + 2 * PT_PI) : p;
+}
+// InfiniteAreaLight::Le (infinite.cpp:92-96)
+__device__ __forceinline__ Spec infinite_le(const DevInfinite &L, const V3 &d) {
+    const V3 w = normalize(xform_vector(L.world_to_light, d));
+    return infinite_lookup(L, spherical_phi(w) * PT_INV_2PI, pt_acosf(pt_clamp(w.z, -1.f, 1.f)) * PT_INV_PI);
+}
+// Distribution1D::SampleContinuous (sampling.h:71-89) over func[n], cdf[n + 1]
+__device__ __forceinline__ float dist1d_sample(const float *func, const float *cdf, float funcInt, int n, float u, float *pdf, int *off) {
+    const int offset = find_interval(cdf, n + 1, u);
+    *off = offset;
+    float du = u - cdf[offset];
+    if ((cdf[offset + 1] - cdf[offset]) > 0) du /= (cdf[offset + 1] - cdf[offset]);
+    *pdf = (funcInt > 0) ? func[offset] / funcInt : 0;
+    return (offset + du) / n;
+}
+// InfiniteAreaLight::Sample_Li (infinite.cpp:98-122) with Distribution2D::SampleContinuous (sampling.h:124-131); *pdf stays 0
+// when the map's pdf is 0.  *pTarget: the point the VisibilityTester aims at.
+__device__ __forceinline__ Spec infinite_sample_li(const DevInfinite &L, const V3 &refP, const float u[2], V3 *wi, float *pdf,
+                                                   V3 *pTarget) {
+    *pdf = 0.f;
+    *wi = *pTarget = mk(0.f, 0.f, 0.f);
+    float pdfs[2];
+    int v, iu;
+    const float d1 = dist1d_sample(L.marg_func, L.marg_cdf, L.marg_func_int, L.nv, u[1], &pdfs[1], &v);
+    const float d0 = dist1d_sample(L.cond_func + (size_t)v * L.nu, L.cond_cdf + (size_t)v * (L.nu + 1), L.cond_func_int[v], L.nu, u[0],
+                                   &pdfs[0], &iu);
+    const float mapPdf = pdfs[0] * pdfs[1];
+    if (mapPdf == 0) return rgb1(0.f);
+    const float theta = d1 * PT_PI, phi = d0 * 2 * PT_PI;
+    const float cosTheta = pt_cosf(theta), sinTheta = pt_sinf(theta);
+    const float sinPhi = pt_sinf(phi), cosPhi = pt_cosf(phi);
+    *wi = xform_vector(L.light_to_world, mk(sinTheta * cosPhi, sinTheta * sinPhi, cosTheta));
+    *pdf = mapPdf / (2 * PT_PI * PT_PI * sinTheta);
+    if (sinTheta == 0) *pdf = 0;
+    *pTarget = refP + *wi * L.two_world_radius;
+    return infinite_lookup(L, d0, d1);
+}
+// InfiniteAreaLight::Pdf_Li (infinite.cpp:124-132; the direction is not normalised) with Distribution2D::Pdf (sampling.h:132-139)
+__device__ __forceinline__ float infinite_pdf_li(const DevInfinite &L, const V3 &w) {
+    const V3 wi = xform_vector(L.world_to_light, w);
+    const float theta = pt_acosf(pt_clamp(wi.z, -1.f, 1.f)), phi = spherical_phi(wi);
+    const float sinTheta = pt_sinf(theta);
+    if (sinTheta == 0) return 0;
+    const float p0 = phi * PT_INV_2PI, p1 = theta * PT_INV_PI;
+    const int iu = pt_mini(pt_maxi(int(p0 * L.nu), 0), L.nu - 1);
+    const int iv = pt_mini(pt_maxi(int(p1 * L.nv), 0), L.nv - 1);
+    return L.cond_func[(size_t)iv * L.nu + iu] / L.marg_func_int / (2 * PT_PI * PT_PI * sinTheta);
+}
+#endif
+
 // ----------------------------------------------------------------------- shade
 struct DirectOut {
     uint32_t pend;
@@ -1117,6 +1191,49 @@ __device__ void estimate_direct(const RenderDev *R, const Isect &is, const Bsdf 
     out->wA = out->pdfA = out->wB = out->pdfB = 0.f;
     out->p1 = out->p1e = out->p1n = mk(0.f, 0.f, 0.f);
     const DevLight &lightRef = R->lights[lightNum];
+#if B200PT_NSPEC == 3
+    if constexpr (VTX) {
+        if (lightRef.kind == B200PT_LIGHT_INFINITE) {
+            // an infinite light (PathIntegrator only: no medium): the shadow ray aims at ref.p + wi * 2 worldRadius like a
+            // point light's, the MIS ray contributes Le(ray) if it hits nothing -- the light's record has tri == B200PT_MISS
+            const DevInfinite &L = R->infinite[lightRef.two_sided];
+            const int flagsNS = BSDF_ALL & ~BSDF_SPECULAR;
+            out->pend = 0;
+            out->sh_o = out->sh_d = out->mi_o = out->mi_d = mk(0.f, 0.f, 0.f);
+            out->A = out->B = rgb1(0.f);
+            V3 wi, pTarget;
+            float lightPdf, scatteringPdf = 0.f;
+            const Spec Li = infinite_sample_li(L, is.p, uLight, &wi, &lightPdf, &pTarget);
+            if (lightPdf > 0 && !is_black(Li)) {
+                const Spec f = bsdf_f<KINDS>(bsdf, is.wo, wi, flagsNS) * absdot(wi, bsdf.ns);
+                scatteringPdf = bsdf_pdf<KINDS>(bsdf, is.wo, wi, flagsNS);
+                if (!is_black(f)) {
+                    const V3 origin = offset_ray_origin(is.p, is.pError, is.n, pTarget - is.p);
+                    out->sh_o = origin;
+                    out->sh_d = pTarget - origin;
+                    const float weight = power_heuristic(lightPdf, scatteringPdf);
+                    out->A = f * Li * weight / lightPdf;
+                    out->pend |= PEND_LIGHT;
+                }
+            }
+            int sampledType = 0;
+            Spec f = bsdf_sample_f<KINDS>(bsdf, is.wo, &wi, uScattering, &scatteringPdf, flagsNS, &sampledType);
+            f = f * absdot(wi, bsdf.ns);
+            if (!is_black(f) && scatteringPdf > 0) {
+                const float lpdf = infinite_pdf_li(L, wi);
+                if (lpdf != 0) {  // `if (lightPdf == 0) return Ld;` (integrator.cpp:182): no MIS ray then
+                    const float weight = power_heuristic(scatteringPdf, lpdf);
+                    const Spec Le = infinite_le(L, wi);
+                    out->B = is_black(Le) ? rgb1(0.f) : f * Le * weight / scatteringPdf;
+                    out->mi_o = offset_ray_origin(is.p, is.pError, is.n, wi);
+                    out->mi_d = wi;
+                    out->pend |= PEND_BSDF;
+                }
+            }
+            return;
+        }
+    }
+#endif
     if (VTX && lightRef.kind != 0) {
         // delta light (scenes with delta lights always run the VTX variant): Sample_Li has pdf 1, there is no MIS weight
         // and no BSDF-sampling branch (integrator.cpp:147-148, :166)
@@ -2460,6 +2577,62 @@ __global__ void __launch_bounds__(256) k_resolve(const RenderDev *R, int bounce,
     }
 }
 
+#if B200PT_NSPEC == 3
+// path.cpp:89-100 for a path ray of `bounce` that found no intersection: at the first vertex or after a specular bounce,
+// L += beta * Le(ray) for each infinite light in Scene::infiniteLights order.  The path ends there (path.cpp:103).
+__global__ void __launch_bounds__(256) k_escape(const RenderDev *R, int bounce, uint32_t *work) {
+    const uint32_t n = R->qcount[bounce * Q_PER_BOUNCE + Q_PATH];
+    const uint32_t *queue = R->q_path[bounce & 1];
+    uint32_t i;
+    while (warp_fetch(work, n, &i)) {
+        if (i >= n) continue;
+        const uint32_t slot = queue[i];
+        PathRec &P = R->path[slot];
+        if (P.hit != B200PT_MISS) continue;
+        const PathVertex v = load_vertex(P);
+        if (!(v.bounces == 0 || v.specularBounce)) continue;
+        float betaW, LW;
+        const Spec beta = ld_spec(P.beta, R->s_beta, slot, &betaW);
+        Spec L = ld_spec(P.L, R->s_L, slot, &LW);
+        for (int k = 0; k < R->n_infinite; ++k) L = L + beta * infinite_le(R->infinite[k], v.rd);
+        st_spec(P.L, R->s_L, slot, L, LW);
+    }
+}
+
+// SpatialLightDistribution::ComputeDistribution's terms of the infinite lights (lightdistrib.cpp:256-275): Li.y() / pdf of
+// Sample_Li at the voxel's 128 Halton points.  Runs after k_spatial_contrib and replaces those lights' entries.
+__global__ void __launch_bounds__(128) k_spatial_infinite(const RenderDev *R) {
+    const SpatialGrid &g = R->grid;
+    const long long nvox = (long long)g.nv[0] * g.nv[1] * g.nv[2];
+    const long long id = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (id >= nvox * R->n_lights) return;
+    const int j = (int)(id % R->n_lights);
+    const DevLight &light = R->lights[j];
+    if (light.kind != B200PT_LIGHT_INFINITE) return;
+    const DevInfinite &L = R->infinite[light.two_sided];
+    const long long vox = id / R->n_lights;
+    const int pi[3] = {(int)(vox % g.nv[0]), (int)((vox / g.nv[0]) % g.nv[1]), (int)(vox / ((long long)g.nv[0] * g.nv[1]))};
+    float lo[3], hi[3];
+    for (int a = 0; a < 3; ++a) {
+        const float t0 = (float)pi[a] / (float)g.nv[a], t1 = (float)(pi[a] + 1) / (float)g.nv[a];
+        const float b0 = lerpf(t0, g.wb_min[a], g.wb_max[a]), b1 = lerpf(t1, g.wb_min[a], g.wb_max[a]);
+        lo[a] = pt_min(b0, b1);
+        hi[a] = pt_max(b0, b1);
+    }
+    float contrib = 0.f;
+    for (int i = 0; i < 128; ++i) {
+        const V3 po = mk(lerpf(radical_inverse(0, i), lo[0], hi[0]), lerpf(radical_inverse(1, i), lo[1], hi[1]),
+                         lerpf(radical_inverse(2, i), lo[2], hi[2]));
+        const float u[2] = {radical_inverse(3, i), radical_inverse(4, i)};
+        V3 wi, pT;
+        float pdf;
+        const Spec Li = infinite_sample_li(L, po, u, &wi, &pdf, &pT);
+        if (pdf > 0) contrib += lum(Li) / pdf;
+    }
+    R->sp_func[vox * R->n_lights + j] = contrib;
+}
+#endif
+
 #if B200PT_NSPEC == 3  // spectrum-independent: compiled once, in the RGBSpectrum translation unit
 // Sobol' byte tables: table[dim][k][b] = XOR of SobolMatrices32[dim*52 + 8k + i] over the set bits i of b.
 __global__ void k_sobol_table(const uint32_t *mat32, uint32_t *table, int n_dims) {
@@ -2865,6 +3038,11 @@ void launch_shade(const RenderDev *dev, int material, bool vertex_data, int boun
 void launch_resolve(const RenderDev *dev, int bounce, uint32_t *work, int grid, cudaStream_t s) {
     B200PT_LAUNCH(B200PT_KERNEL(k_resolve), grid, 256, s, dev, bounce, work);
 }
+#if B200PT_NSPEC == 3
+void launch_escape(const RenderDev *dev, int bounce, uint32_t *work, int grid, cudaStream_t s) {
+    B200PT_LAUNCH(B200PT_KERNEL(k_escape), grid, 256, s, dev, bounce, work);
+}
+#endif
 
 void launch_medium(const RenderDev *dev, int bounce, uint32_t *work, int grid, cudaStream_t s) {
     B200PT_LAUNCH(B200PT_KERNEL(k_medium), grid, 128, s, dev, bounce, work);
@@ -2890,6 +3068,9 @@ void launch_spatial_build(const RenderDev *dev, const RenderDev &host, cudaStrea
     const long long nvox = (long long)host.grid.nv[0] * host.grid.nv[1] * host.grid.nv[2];
     const long long n1 = nvox * host.n_lights;
     B200PT_LAUNCH(B200PT_KERNEL(k_spatial_contrib), (unsigned)((n1 + 127) / 128), 128, s, dev);
+#if B200PT_NSPEC == 3
+    if (host.n_infinite > 0) B200PT_LAUNCH(B200PT_KERNEL(k_spatial_infinite), (unsigned)((n1 + 127) / 128), 128, s, dev);
+#endif
     B200PT_LAUNCH(B200PT_KERNEL(k_spatial_cdf), (unsigned)((nvox + 127) / 128), 128, s, dev);
 }
 

@@ -33,6 +33,20 @@ struct DevLight {
     float two_world_radius;
 };
 
+// InfiniteAreaLight (b200pt_infinite_light): level 0 of the map and the host's Distribution2D tables.  Its DevLight
+// record keeps kind, tri = B200PT_MISS and, in two_sided, the index into RenderDev::infinite.
+struct DevInfinite {
+    int w, h;                 // level-0 texels [h][w] (RGB, float4 each)
+    const float4 *texels;
+    float light_to_world[16];
+    float world_to_light[16];
+    int nu, nv;
+    const float *cond_func, *cond_cdf, *cond_func_int;  // [nv][nu], [nv][nu + 1], [nv]
+    const float *marg_func, *marg_cdf;                  // [nv], [nv + 1]
+    float marg_func_int;
+    float two_world_radius;
+};
+
 struct DevScene {
     const U4 *nodes;
     const uint32_t *tri_base;  // per node: first triangle of its leaf children (wbvh.h)
@@ -64,6 +78,7 @@ enum {
     W_SPHERES_SHADOW = 9,
     W_SPHERES_MIS = 10,
     W_MEDIUM = 11,
+    W_ESCAPE = 12,         // escaped path rays of scenes with infinite lights (k_escape)
     W_PER_BOUNCE = 16
 };
 // bounded media: the counters of the boundary passes inside a bounce (zeroed between passes, see b200pt_render_tiles)
@@ -183,6 +198,10 @@ struct RenderDev {
     float4 *sh_tr, *mi_tr;     // transmittance so far along the shadow / MIS ray, medium id of the current segment (bits)
     float4 *sh_p1, *sh_p1e, *sh_p1n;  // the light sample the shadow ray is re-aimed at after each boundary (SpawnRayTo)
     unsigned long long *dim_overflows;  // paths ended because their sampler dimension ran past the host's tables
+    // infinite area lights (DevLight::kind == B200PT_LIGHT_INFINITE, DevLight::two_sided = index into `infinite`), in
+    // Scene::infiniteLights order; scenes with n_infinite > 0 run the full shading variant (RGB build only)
+    const DevInfinite *infinite;
+    int n_infinite;
 };
 
 // resident CTAs of k_trace per SM (128 threads each).  7 (up to 72 registers, no spills) measured fastest on the H100
@@ -249,6 +268,9 @@ void launch_spheres(const TraceArgs &a, bool any_hit, bool classify, int grid, c
 void launch_shade(const RenderDev *dev, int material, bool vertex_data, int bounce, uint32_t *work, int grid,
                   cudaStream_t s);
 void launch_resolve(const RenderDev *dev, int bounce, uint32_t *work, int grid, cudaStream_t s);
+// Scenes with infinite lights: L += beta * Le(ray) of every infinite light for the path rays of `bounce` that hit nothing,
+// at the first vertex or after a specular bounce (path.cpp:89-100).  After resolve(bounce - 1), before shade(bounce + 1).
+void launch_escape(const RenderDev *dev, int bounce, uint32_t *work, int grid, cudaStream_t s);
 // Medium pass of a bounce (scenes inside a homogeneous medium): after the closest-hit launch, before the shading kernels.
 void launch_medium(const RenderDev *dev, int bounce, uint32_t *work, int grid, cudaStream_t s);
 // Scenes with bounded media: one pass of the medium kernel over `queue` (the bounce's path queue, then the rays that crossed

@@ -1617,9 +1617,8 @@ B200_HD float power_heuristic(float fPdf, float gPdf) {
     float f = fPdf, g = gPdf;
     return (f * f) / (f * f + g * g);
 }
-// pbrt.h:353-368 FindInterval over cdf[0..n] + sampling.h:90-100
-B200_HD int sample_discrete(const float *cdf, const float *func, float funcInt, int n, float u, float *pdf) {
-    int size = n + 1;
+// pbrt.h:353-368 FindInterval over cdf[0..size-1] with the predicate cdf[i] <= u
+B200_HD int find_interval(const float *cdf, int size, float u) {
     int first = 0, l = size;
     while (l > 0) {
         int half = l >> 1, middle = first + half;
@@ -1629,7 +1628,11 @@ B200_HD int sample_discrete(const float *cdf, const float *func, float funcInt, 
         } else
             l = half;
     }
-    int offset = pt_mini(pt_maxi(first - 1, 0), size - 2);
+    return pt_mini(pt_maxi(first - 1, 0), size - 2);
+}
+// sampling.h:90-100 over cdf[0..n]
+B200_HD int sample_discrete(const float *cdf, const float *func, float funcInt, int n, float u, float *pdf) {
+    int offset = find_interval(cdf, n + 1, u);
     *pdf = (funcInt > 0) ? func[offset] / (funcInt * n) : 0.f;
     return offset;
 }

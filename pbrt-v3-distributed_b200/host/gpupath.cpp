@@ -73,6 +73,7 @@
 #include "lights/spot.h"
 #include "lights/point.h"
 #include "lights/distant.h"
+#include "lights/infinite.h"
 #include "materials/glass.h"
 #include "materials/matte.h"
 #include "materials/metal.h"
@@ -158,6 +159,14 @@ struct Flattened {
     // into boundedMedia (the medium inside) or -1; boundaryOutside[k] is what the scene declares outside boundary medium k
     std::vector<int32_t> sphereMedium;
     std::vector<const Medium *> boundedMedia, boundaryOutside;
+    // InfiniteAreaLights: what b200pt_scene_set_infinite_light takes, copied from the light's own members
+    struct Infinite {
+        int light;
+        int width, height, nu, nv;
+        std::vector<float> texels, condFunc, condCdf, condFuncInt, margFunc, margCdf;
+        float margFuncInt, lightToWorld[16], powerRGB[3];
+    };
+    std::vector<Infinite> infinite;
 };
 
 // materials/{matte,plastic,metal,glass}.cpp ComputeScatteringFunctions with constant textures
@@ -434,7 +443,9 @@ bool FlattenScene(const Scene &scene, Flattened *f, std::string *why, bool volum
             }
         }
     }
-    if (!scene.infiniteLights.empty()) return *why = "infinite area lights", false;
+    // Spectrum(RGBSpectrum, Illuminant) is a per-lookup FromRGB on SampledSpectrum hosts, which the device does not restate
+    if (!scene.infiniteLights.empty() && kSampledHost) return *why = "infinite area lights in a SampledSpectrum build", false;
+    if (!scene.infiniteLights.empty() && volumetric) return *why = "infinite area lights under the volumetric integrator", false;
     for (size_t l = 0; l < scene.lights.size(); ++l) {
         b200pt_area_light bl;
         memset(&bl, 0, sizeof(bl));
@@ -465,8 +476,39 @@ bool FlattenScene(const Scene &scene, Flattened *f, std::string *why, bool volum
             f->lights.push_back(bl);
             continue;
         }
+        if (auto il = dynamic_cast<const InfiniteAreaLight *>(scene.lights[l].get())) {
+            // infinite.cpp:43-84: level 0 of Lmap (Le and Sample_Li look it up with width 0), the Distribution2D as built
+            bl.kind = B200PT_LIGHT_INFINITE;
+            memcpy(bl.world_to_light, il->WorldToLight.m.m, sizeof(float) * 16);
+            bl.world_radius = il->worldRadius;  // set by InfiniteAreaLight::Preprocess in the Scene constructor
+            Flattened::Infinite in;
+            in.light = (int)l;
+            const auto &lv0 = *il->Lmap->pyramid[0];
+            in.width = lv0.uSize();
+            in.height = lv0.vSize();
+            for (int t = 0; t < in.height; ++t)
+                for (int s = 0; s < in.width; ++s)
+                    for (int c = 0; c < 3; ++c) in.texels.push_back(lv0(s, t)[c]);
+            const Distribution2D &d2 = *il->distribution;
+            in.nv = (int)d2.pConditionalV.size();
+            in.nu = d2.pConditionalV[0]->Count();
+            for (const auto &row : d2.pConditionalV) {
+                in.condFunc.insert(in.condFunc.end(), row->func.begin(), row->func.end());
+                in.condCdf.insert(in.condCdf.end(), row->cdf.begin(), row->cdf.end());
+                in.condFuncInt.push_back(row->funcInt);
+            }
+            in.margFunc = d2.pMarginal->func;
+            in.margCdf = d2.pMarginal->cdf;
+            in.margFuncInt = d2.pMarginal->funcInt;
+            memcpy(in.lightToWorld, il->LightToWorld.m.m, sizeof(float) * 16);
+            const RGBSpectrum pw = il->Lmap->Lookup(Point2f(.5f, .5f), .5f);
+            for (int c = 0; c < 3; ++c) in.powerRGB[c] = pw[c];
+            f->infinite.push_back(std::move(in));
+            f->lights.push_back(bl);
+            continue;
+        }
         auto dl = dynamic_cast<const DiffuseAreaLight *>(scene.lights[l].get());
-        if (!dl) return *why = "a light other than diffuse area / point / spot / distant lights", false;
+        if (!dl) return *why = "a light other than diffuse area / point / spot / distant / infinite lights", false;
         ToRGB(dl->Lemit, bl.lemit, &f->lightSpectra);
         bl.two_sided = dl->twoSided ? 1 : 0;
         auto is = sphereOfShape.find(dl->shape.get());
@@ -688,6 +730,20 @@ class GpuIntegrator : public Base {
                     fwrite(sd.light_spectra, 4, (size_t)sd.n_lights * ns, df);
                     fwrite(sd.cie_xyz, 4, (size_t)3 * ns, df);
                 }
+                // infinite lights (appended after the layout above): light index, map and distribution sizes, the tables
+                for (const auto &in : flat.infinite) {
+                    const int32_t sz[5] = {in.light, in.width, in.height, in.nu, in.nv};
+                    fwrite(sz, 4, 5, df);
+                    fwrite(in.texels.data(), 4, in.texels.size(), df);
+                    fwrite(in.lightToWorld, 4, 16, df);
+                    fwrite(in.condFunc.data(), 4, in.condFunc.size(), df);
+                    fwrite(in.condCdf.data(), 4, in.condCdf.size(), df);
+                    fwrite(in.condFuncInt.data(), 4, in.condFuncInt.size(), df);
+                    fwrite(in.margFunc.data(), 4, in.margFunc.size(), df);
+                    fwrite(in.margCdf.data(), 4, in.margCdf.size(), df);
+                    fwrite(&in.margFuncInt, 4, 1, df);
+                    fwrite(in.powerRGB, 4, 3, df);
+                }
                 fclose(df);
             }
         }
@@ -714,6 +770,24 @@ class GpuIntegrator : public Base {
         B200_CHECK(b200pt_ctx_create(device, &ctx));
         const auto t1 = now();
         B200_CHECK(b200pt_scene_create(ctx, &sd, &gscene));
+        for (const auto &in : flat.infinite) {
+            b200pt_infinite_light il;
+            memset(&il, 0, sizeof(il));
+            il.width = in.width;
+            il.height = in.height;
+            il.texels = in.texels.data();
+            memcpy(il.light_to_world, in.lightToWorld, sizeof(il.light_to_world));
+            il.nu = in.nu;
+            il.nv = in.nv;
+            il.cond_func = in.condFunc.data();
+            il.cond_cdf = in.condCdf.data();
+            il.cond_func_int = in.condFuncInt.data();
+            il.marg_func = in.margFunc.data();
+            il.marg_cdf = in.margCdf.data();
+            il.marg_func_int = in.margFuncInt;
+            memcpy(il.power_rgb, in.powerRGB, sizeof(il.power_rgb));
+            B200_CHECK(b200pt_scene_set_infinite_light(gscene, in.light, &il));
+        }
         B200_CHECK(b200pt_render_create(gscene, &cd, &fd, &smpd, &id, &render));
         B200_CHECK(b200pt_ctx_synchronize(ctx));
         const auto t2 = now();

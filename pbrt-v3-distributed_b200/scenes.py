@@ -139,7 +139,7 @@ class SceneArrays:
 
     def __init__(self, n_tris, materials=("matte",), soup_version=1, seed=1234, light_L=40.0,
                  n_lights=None, two_sided=False, reverse_orientation=(), shading_normals=(), uvs=(), spheres=(),
-                 objects=(), instances=(), delta_lights=()):
+                 objects=(), instances=(), delta_lights=(), infinite_lights=()):
         """spheres: dicts {center, radius, material (a name in `materials` or "black"), emit (radiance or
         None), scale (sx, sy, sz) or None, reverse_orientation} -- written as `Translate` + `Scale` +
         `Shape "sphere"` by write_pbrt, after the meshes."""
@@ -218,7 +218,10 @@ class SceneArrays:
         # delta lights: dicts {kind: "point"|"spot"|"distant", from_, to, I or L, coneangle, conedelta}; they follow
         # the emissive quads in the .pbrt file, hence in Scene::lights
         self.delta_specs = [dict(x) for x in delta_lights]
-        self._lights = (abi.AreaLight * max(nl + len(self.delta_specs) + n_sl, 1))()
+        # infinite lights: dicts {L (rgb or scalar), scale (rgb or scalar), map (array [h][w][3], written as <name>_sky<k>.pfm
+        # and named by "string mapname") or None, steps: [(op, args)] of the light's transform}; they follow the delta lights
+        self.infinite_specs = [dict(x) for x in infinite_lights]
+        self._lights = (abi.AreaLight * max(nl + len(self.delta_specs) + len(self.infinite_specs) + n_sl, 1))()
         for i in range(nl):
             self._lights[i].triangle = i
             self._lights[i].lemit[:] = [light_L] * 3
@@ -244,6 +247,12 @@ class SceneArrays:
                 ln = np.sqrt(f32(f32(f32(dvec[0] * dvec[0]) + f32(dvec[1] * dvec[1])) + f32(dvec[2] * dvec[2])))
                 inv = f32(1) / f32(ln)  # Vector3::operator/ multiplies by the reciprocal (geometry.h:132-137)
                 rec.position[:] = [f32(v * inv) for v in dvec]
+        for il in self.infinite_specs:  # CreateInfiniteLight (infinite.cpp:180-191): WorldToLight = Inverse(CTM)
+            rec = self._lights[nl]
+            nl += 1
+            rec.triangle, rec.sphere, rec.kind = -1, -1, abi.LIGHT_INFINITE
+            _, minv = ctm(il.get("steps", ()))
+            rec.world_to_light[:] = minv.reshape(-1).tolist()
         self._spheres = (abi.Sphere * max(len(self.sphere_specs), 1))()
         for k, sp in enumerate(self.sphere_specs):
             m, minv = sphere_transform(sp["center"], sp.get("scale"))
@@ -489,6 +498,17 @@ def write_pbrt(dirname, name, scene, xres, yres, spp, max_depth=5, strategy="uni
         else:
             lines.append('LightSource "distant" "rgb L" [%s] "point from" [%.9g %.9g %.9g] "point to" [%.9g %.9g %.9g]'
                          % ((rgb,) + tuple(f_) + tuple(t_)))
+    for k, il in enumerate(getattr(scene, "infinite_specs", ())):
+        rgb3 = lambda v: "%.9g %.9g %.9g" % ((v,) * 3 if np.isscalar(v) else tuple(v))
+        light = 'LightSource "infinite" "rgb L" [%s]' % rgb3(il.get("L", 1.0))
+        if "scale" in il:
+            light += ' "rgb scale" [%s]' % rgb3(il["scale"])
+        if il.get("map") is not None:
+            sky = "%s_sky%d.pfm" % (name, k)
+            write_pfm(os.path.join(dirname, sky), np.asarray(il["map"], np.float32))
+            light += ' "string mapname" "%s"' % sky
+        lines += ["AttributeBegin"] + ["  %s %s" % (op, " ".join("%.9g" % v for v in args)) for op, args in il.get("steps", ())]
+        lines += ["  " + light, "AttributeEnd"]
     for m, part in enumerate(scene.ply_parts):
         ply = "%s_m%d.ply" % (name, m)
         sel = scene.material_id == m
@@ -535,6 +555,36 @@ def write_pbrt(dirname, name, scene, xres, yres, spp, max_depth=5, strategy="uni
     with open(path, "w") as f:
         f.write("\n".join(lines) + "\n")
     return path
+
+
+def read_dump_infinite(path, abi):
+    """{light index: tables for Scene.set_infinite_light} of the InfiniteAreaLights an RGBSpectrum host wrote to its
+    B200PT_DUMP_SCENE file (host/gpupath.cpp appends them after the descriptors)."""
+    raw = open(path, "rb").read()
+    hdr = np.frombuffer(raw, np.int64, 8)
+    nt, nm, nl, nsph, has_n, has_uv = (int(x) for x in hdr[1:7])
+    off = 64 + nt * (36 + 4 + 4 + 1 + 1) + (nt * 36 if has_n else 0) + (nt * 24 if has_uv else 0)
+    off += nm * C.sizeof(abi.Material) + nl * C.sizeof(abi.AreaLight) + nsph * C.sizeof(abi.Sphere)
+    off += C.sizeof(abi.CameraDesc) + 48 + C.sizeof(abi.IntegratorDesc) + 24  # film desc (48 B), six sampler ints
+    if int(np.frombuffer(raw, np.int32, 1, off)[0]) != 0:
+        raise ValueError("%s: not an RGBSpectrum host's dump" % path)
+    off += 4
+    out = {}
+
+    def take(n, shape=None):
+        nonlocal off
+        a = np.frombuffer(raw, np.float32, n, off).copy()
+        off += 4 * n
+        return a.reshape(shape) if shape else a
+    while off < len(raw):
+        light, w, h, nu, nv = (int(x) for x in np.frombuffer(raw, np.int32, 5, off))
+        off += 20
+        out[light] = dict(texels=take(w * h * 3, (h, w, 3)), light_to_world=take(16), cond_func=take(nv * nu, (nv, nu)),
+                          cond_cdf=take(nv * (nu + 1), (nv, nu + 1)), cond_func_int=take(nv), marg_func=take(nv),
+                          marg_cdf=take(nv + 1), marg_func_int=take(1)[0], power_rgb=take(3))
+    if off != len(raw):
+        raise ValueError("%s: truncated infinite-light tables" % path)
+    return out
 
 
 def read_pfm(path):
