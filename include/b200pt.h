@@ -11,8 +11,9 @@
  * (core/film.h:121-161, core/film.cpp:117-130).  Widened since (each descriptor
  * says where): the Halton sampler, Sphere shapes and sphere lights, object
  * instances, the mirror material, point / spot / distant lights, every pixel
- * filter, SampledSpectrum hosts (60-bin spectra), and VolPathIntegrator
- * (integrators/volpath.cpp:60-188) with one homogeneous medium around the scene.
+ * filter, SampledSpectrum hosts (60-bin spectra), VolPathIntegrator
+ * (integrators/volpath.cpp:60-188) with one homogeneous medium around the scene,
+ * infinite area lights, and image textures (textures/imagemap.h) on RGB hosts.
  *
  * The reference has no FFI: its "plugins" are C++ subclasses picked by name in
  * RenderOptions::MakeIntegrator (core/api.cpp:1666-1718).  A host integrator
@@ -64,10 +65,13 @@ typedef enum b200pt_material_type {
     B200PT_MAT_NONE = 4     /* null material: GetMaterial()==nullptr is NOT supported; reserved */
 } b200pt_material_type;
 
-/* Textures are constant (textures/constant.h); the host evaluates them and
+/* Constant textures (textures/constant.h) are evaluated by the host, which also
  * applies TrowbridgeReitzDistribution::RoughnessToAlpha (microfacet.h:123-128)
  * itself, so alpha_x/alpha_y below are the final alphas. Spectra are RGB
- * (core/spectrum.h:429), already Clamp()ed like the materials do. */
+ * (core/spectrum.h:429), already Clamp()ed like the materials do.  On RGBSpectrum
+ * hosts a parameter may instead be an ImageTexture under UVMapping2D
+ * (b200pt_scene_bind_texture): the device then evaluates it per hit, clamps and
+ * remaps it like the material does, and the value here is ignored. */
 typedef struct b200pt_material {
     int32_t type;        /* b200pt_material_type */
     float kd[3];         /* matte Kd, plastic Kd                      */
@@ -378,6 +382,37 @@ typedef struct b200pt_infinite_light {
 /* Sets the map and tables of light `light` (kind B200PT_LIGHT_INFINITE) of the scene; the library copies them.  Call it
  * between b200pt_scene_create and b200pt_render_create, once per infinite light. */
 int b200pt_scene_set_infinite_light(b200pt_scene *scene, int32_t light, const b200pt_infinite_light *desc);
+
+/* ---- image textures: ImageTexture (textures/imagemap.h) under UVMapping2D (core/texture.cpp:93-99), RGBSpectrum hosts.
+ * A MIPMap (core/mipmap.h) is uploaded once as the host built it -- every pyramid level (after the host's power-of-two
+ * resampling, "scale" and "gamma"), its wrap mode, filter settings and MIPMap::weightLut -- and bound to any number of
+ * (material, parameter) slots, each with its own mapping.  The device filters it with the camera ray's differentials
+ * (SurfaceInteraction::ComputeDifferentials, interaction.cpp:103-149) exactly like MIPMap::Lookup(st, dst0, dst1). */
+enum { B200PT_WRAP_REPEAT = 0, B200PT_WRAP_BLACK = 1, B200PT_WRAP_CLAMP = 2 };  /* ImageWrap (mipmap.h:47) */
+#define B200PT_MIPMAP_MAX_LEVELS 16
+typedef struct b200pt_mipmap {
+    int32_t n_levels;               /* pyramid.size(): 1 + Log2Int(max(width, height)) of level 0                     */
+    int32_t channels;               /* 3 (spectrum texture, RGB texels) or 1 (float texture)                          */
+    int32_t width[B200PT_MIPMAP_MAX_LEVELS], height[B200PT_MIPMAP_MAX_LEVELS];  /* uSize(), vSize() of every level:
+                                       powers of two, each level max(1, previous / 2)                                  */
+    const float *texels[B200PT_MIPMAP_MAX_LEVELS];  /* [height][width][channels] of every level                        */
+    int32_t wrap;                   /* B200PT_WRAP_*                                                                  */
+    int32_t trilinear;              /* MIPMap::doTrilinear                                                            */
+    float max_anisotropy;           /* MIPMap::maxAnisotropy                                                          */
+    float weight_lut[128];          /* MIPMap::weightLut                                                              */
+} b200pt_mipmap;
+/* Material parameter slots a texture can be bound to, and the material types that have them:
+ *   KD: matte, plastic   KS: plastic Ks, glass Kr, mirror Kr   KT: glass Kt   ETA, K: metal
+ *   ROUGHNESS_U: plastic roughness (both alphas), metal uroughness (or roughness)   ROUGHNESS_V: metal vroughness (or
+ *   roughness).  Spectrum slots take 3-channel maps, the roughness slots 1-channel maps. */
+enum { B200PT_TEX_KD = 0, B200PT_TEX_KS = 1, B200PT_TEX_KT = 2, B200PT_TEX_ETA = 3, B200PT_TEX_K = 4,
+       B200PT_TEX_ROUGHNESS_U = 5, B200PT_TEX_ROUGHNESS_V = 6, B200PT_TEX_SLOTS = 7 };
+/* Copies the pyramid to the device; *id names it in b200pt_scene_bind_texture. */
+int b200pt_scene_add_mipmap(b200pt_scene *scene, const b200pt_mipmap *desc, int32_t *id);
+/* Binds MIPMap `mipmap` with UVMapping2D(su, sv, du, dv) to parameter `slot` of material `material`.  remap_roughness:
+ * the material's "remaproughness" (roughness slots only: the looked-up value goes through RoughnessToAlpha). */
+int b200pt_scene_bind_texture(b200pt_scene *scene, int32_t material, int32_t slot, int32_t mipmap, float su, float sv,
+                              float du, float dv, int32_t remap_roughness);
 
 /* ---- kernel-level entry points (parity tests, traversal benchmarks) -------
  * Replace Scene::Intersect / Scene::IntersectP (core/scene.cpp:45-55) on

@@ -42,6 +42,8 @@ _SIGNATURES = {
     "b200pt_scene_upload": (C.c_int, [_vp, C.POINTER(_u64)]),
     "b200pt_scene_info": (C.c_int, [_vp, C.POINTER(_u64), C.POINTER(_u64), C.POINTER(_u64)]),
     "b200pt_scene_set_infinite_light": (C.c_int, [_vp, _i32, C.POINTER(abi.InfiniteLight)]),
+    "b200pt_scene_add_mipmap": (C.c_int, [_vp, C.POINTER(abi.Mipmap), C.POINTER(_i32)]),
+    "b200pt_scene_bind_texture": (C.c_int, [_vp, _i32, _i32, _i32, C.c_float, C.c_float, C.c_float, C.c_float, _i32]),
     "b200pt_trace_closest": (C.c_int, [_vp, _vp, _vp, _i64]),
     "b200pt_trace_any": (C.c_int, [_vp, _vp, _vp, _i64]),
     "b200pt_trace_closest_dev": (C.c_int, [_vp, _u64, _u64, _i64]),
@@ -187,6 +189,28 @@ class Scene:
         rec.marg_func_int = float(np.float32(tables["marg_func_int"]))
         rec.power_rgb[:] = [float(v) for v in f32("power_rgb")]
         _check(lib.b200pt_scene_set_infinite_light(self.h, int(light), C.byref(rec)))
+
+    def add_mipmap(self, levels, wrap, trilinear, max_anisotropy, weight_lut):
+        """b200pt_scene_add_mipmap: `levels` are the pyramid's texel arrays, [h][w][3] (spectrum) or [h][w] (float);
+        returns the MIPMap's id.  The library copies the texels."""
+        arrs = [np.ascontiguousarray(a, dtype=np.float32) for a in levels]
+        rec = abi.Mipmap()
+        rec.n_levels = len(arrs)
+        rec.channels = 3 if arrs[0].ndim == 3 else 1
+        for i, a in enumerate(arrs[:abi.MIPMAP_MAX_LEVELS]):
+            rec.height[i], rec.width[i] = a.shape[:2]
+            rec.texels[i] = a.ctypes.data
+        rec.wrap, rec.trilinear, rec.max_anisotropy = int(wrap), int(trilinear), float(max_anisotropy)
+        rec.weight_lut[:] = [float(v) for v in np.asarray(weight_lut, dtype=np.float32)]
+        out = _i32()
+        _check(lib.b200pt_scene_add_mipmap(self.h, C.byref(rec), C.byref(out)))
+        return out.value
+
+    def bind_texture(self, material, slot, mipmap, su=1.0, sv=1.0, du=0.0, dv=0.0, remap_roughness=False):
+        """b200pt_scene_bind_texture: MIPMap `mipmap` under UVMapping2D(su, sv, du, dv) on parameter `slot` (abi.TEX_*)
+        of material `material`."""
+        _check(lib.b200pt_scene_bind_texture(self.h, int(material), int(slot), int(mipmap), su, sv, du, dv,
+                                             1 if remap_roughness else 0))
 
     def trace_closest(self, rays):
         rays = np.ascontiguousarray(rays, dtype=abi.RAY_DTYPE)

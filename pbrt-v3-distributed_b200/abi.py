@@ -75,6 +75,18 @@ class InfiniteLight(C.Structure):
                 ("marg_func_int", C.c_float), ("power_rgb", C.c_float * 3)]
 
 
+WRAP_REPEAT, WRAP_BLACK, WRAP_CLAMP = 0, 1, 2  # B200PT_WRAP_*
+MIPMAP_MAX_LEVELS = 16
+TEX_KD, TEX_KS, TEX_KT, TEX_ETA, TEX_K, TEX_ROUGHNESS_U, TEX_ROUGHNESS_V, TEX_SLOTS = range(8)
+
+
+class Mipmap(C.Structure):
+    """b200pt_mipmap: an ImageTexture's MIPMap as the host built it (every level, wrap, filter settings, weightLut)."""
+    _fields_ = [("n_levels", C.c_int32), ("channels", C.c_int32), ("width", C.c_int32 * MIPMAP_MAX_LEVELS),
+                ("height", C.c_int32 * MIPMAP_MAX_LEVELS), ("texels", C.c_void_p * MIPMAP_MAX_LEVELS), ("wrap", C.c_int32),
+                ("trilinear", C.c_int32), ("max_anisotropy", C.c_float), ("weight_lut", C.c_float * 128)]
+
+
 class SamplerDesc(C.Structure):
     _fields_ = [("samples_per_pixel", C.c_int32), ("sample_bounds", C.c_int32 * 4),
                 ("n_dimensions", C.c_int32), ("matrices32", C.c_void_p), ("vdc", C.c_void_p),

@@ -42,7 +42,8 @@ struct b200pt_ctx {
 // over its own RenderDev objects (render_dev_size() is checked once per render object).
 namespace b200pt_s60 {
 struct RenderDev;
-void launch_raygen(const RenderDev *dev, uint32_t batch_first_tile, uint32_t n_batch_tiles, uint32_t n_slots, cudaStream_t s);
+void launch_raygen(const RenderDev *dev, uint32_t batch_first_tile, uint32_t n_batch_tiles, uint32_t n_slots, bool keep_pfilm,
+                   cudaStream_t s);
 void launch_shade(const RenderDev *dev, int material, bool vertex_data, int bounce, uint32_t *work, int grid, cudaStream_t s);
 void launch_resolve(const RenderDev *dev, int bounce, uint32_t *work, int grid, cudaStream_t s);
 void launch_medium(const RenderDev *dev, int bounce, uint32_t *work, int grid, cudaStream_t s);
@@ -89,6 +90,12 @@ struct b200pt_scene {
     std::vector<float> infinite_power;  // [n_lights][3]
     std::vector<char> infinite_set;
     std::vector<void *> d_infinite_tables;
+    // image textures (b200pt_scene_add_mipmap / b200pt_scene_bind_texture): the MIPMaps (level pointers into
+    // d_mipmap_texels[id]) and, once a texture is bound, [n_materials][B200PT_TEX_SLOTS] bindings
+    std::vector<DevMipmap> mipmaps;
+    std::vector<int> mipmap_channels;
+    std::vector<void *> d_mipmap_texels;
+    std::vector<DevTexBind> tex_bind;
 };
 
 struct TimedLaunch {
@@ -703,6 +710,7 @@ void b200pt_scene_destroy(b200pt_scene *s) {
     cudaFree(s->d_instances);
     cudaFree(s->d_work);
     for (void *p : s->d_infinite_tables) cudaFree(p);
+    for (void *p : s->d_mipmap_texels) cudaFree(p);
     cudaFreeHost(s->h_nodes);
     cudaFreeHost(s->h_tri_base);
     cudaFreeHost(s->h_tris);
@@ -762,6 +770,110 @@ int b200pt_scene_set_infinite_light(b200pt_scene *s, int32_t light, const b200pt
     L.marg_func_int = d->marg_func_int;
     memcpy(&s->infinite_power[3 * (size_t)light], d->power_rgb, 3 * sizeof(float));
     s->infinite_set[light] = 1;
+    return B200PT_OK;
+}
+
+int b200pt_scene_add_mipmap(b200pt_scene *s, const b200pt_mipmap *d, int32_t *id) {
+    if (!s || !d || !id) return b200pt_fail(B200PT_ERR_INVALID, "scene_add_mipmap: NULL argument");
+    if (s->nspec) return b200pt_fail(B200PT_ERR_INVALID, "scene_add_mipmap: image textures are not supported for SampledSpectrum hosts");
+    const int nl = d->n_levels;
+    if (nl < 1 || nl > B200PT_MIPMAP_MAX_LEVELS)
+        return b200pt_fail(B200PT_ERR_INVALID, "scene_add_mipmap: %d levels (1 to %d)", nl, B200PT_MIPMAP_MAX_LEVELS);
+    if (d->channels != 1 && d->channels != 3) return b200pt_fail(B200PT_ERR_INVALID, "scene_add_mipmap: %d channels (1 or 3)", d->channels);
+    if (d->wrap < B200PT_WRAP_REPEAT || d->wrap > B200PT_WRAP_CLAMP)
+        return b200pt_fail(B200PT_ERR_INVALID, "scene_add_mipmap: unknown wrap mode %d", d->wrap);
+    // MIPMap's constructor (mipmap.h:184-207): power-of-two level 0 with 1 + Log2Int(max(w, h)) levels, each halving
+    const int w0 = d->width[0], h0 = d->height[0];
+    auto pow2 = [](int v) { return v > 0 && (v & (v - 1)) == 0; };
+    if (!pow2(w0) || !pow2(h0) || w0 > (1 << (B200PT_MIPMAP_MAX_LEVELS - 1)) || h0 > (1 << (B200PT_MIPMAP_MAX_LEVELS - 1)))
+        return b200pt_fail(B200PT_ERR_INVALID, "scene_add_mipmap: level 0 is %d x %d, not powers of two up to %d", w0, h0,
+                           1 << (B200PT_MIPMAP_MAX_LEVELS - 1));
+    int log2max = 0;
+    while ((1 << (log2max + 1)) <= std::max(w0, h0)) ++log2max;
+    if (nl != 1 + log2max) return b200pt_fail(B200PT_ERR_INVALID, "scene_add_mipmap: %d levels for a %d x %d map (want %d)", nl, w0, h0, 1 + log2max);
+    size_t total = 0;
+    for (int l = 0; l < nl; ++l) {
+        const int ew = l ? std::max(1, d->width[l - 1] / 2) : w0, eh = l ? std::max(1, d->height[l - 1] / 2) : h0;
+        if (d->width[l] != ew || d->height[l] != eh)
+            return b200pt_fail(B200PT_ERR_INVALID, "scene_add_mipmap: level %d is %d x %d (want %d x %d)", l, d->width[l], d->height[l], ew, eh);
+        if (!d->texels[l]) return b200pt_fail(B200PT_ERR_INVALID, "scene_add_mipmap: texels of level %d are NULL", l);
+        total += (size_t)ew * eh;
+    }
+    if (!(d->max_anisotropy == d->max_anisotropy)) return b200pt_fail(B200PT_ERR_INVALID, "scene_add_mipmap: maxanisotropy is NaN");
+    CUDA_TRY(cudaSetDevice(s->ctx->device));
+    std::vector<float4> h(total);
+    DevMipmap M;
+    memset(&M, 0, sizeof(M));
+    M.levels = nl;
+    M.wrap = d->wrap;
+    M.trilinear = d->trilinear ? 1 : 0;
+    M.max_aniso = d->max_anisotropy;
+    memcpy(M.weight_lut, d->weight_lut, sizeof(M.weight_lut));
+    size_t off[B200PT_MIPMAP_MAX_LEVELS], o = 0;
+    for (int l = 0; l < nl; ++l) {
+        off[l] = o;
+        M.w[l] = d->width[l];
+        M.h[l] = d->height[l];
+        const size_t n = (size_t)M.w[l] * M.h[l];
+        for (size_t i = 0; i < n; ++i) {
+            const float *t = d->texels[l] + i * d->channels;
+            h[o + i] = d->channels == 3 ? make_float4(t[0], t[1], t[2], 0.f) : make_float4(t[0], t[0], t[0], 0.f);
+        }
+        o += n;
+    }
+    float4 *dp = nullptr;
+    if (cudaMalloc(&dp, total * sizeof(float4)) != cudaSuccess)
+        return b200pt_fail(B200PT_ERR_OOM, "scene_add_mipmap: cudaMalloc of %zu bytes failed", total * sizeof(float4));
+    if (cudaMemcpy(dp, h.data(), total * sizeof(float4), cudaMemcpyHostToDevice) != cudaSuccess) {
+        cudaFree(dp);
+        return b200pt_fail(B200PT_ERR_CUDA, "scene_add_mipmap: upload failed");
+    }
+    for (int l = 0; l < nl; ++l) M.texels[l] = dp + off[l];
+    *id = (int32_t)s->mipmaps.size();
+    s->mipmaps.push_back(M);
+    s->mipmap_channels.push_back(d->channels);
+    s->d_mipmap_texels.push_back(dp);
+    return B200PT_OK;
+}
+
+int b200pt_scene_bind_texture(b200pt_scene *s, int32_t material, int32_t slot, int32_t mipmap, float su, float sv, float du, float dv,
+                              int32_t remap_roughness) {
+    if (!s) return b200pt_fail(B200PT_ERR_INVALID, "scene_bind_texture: scene is NULL");
+    if (s->nspec) return b200pt_fail(B200PT_ERR_INVALID, "scene_bind_texture: image textures are not supported for SampledSpectrum hosts");
+    if (material < 0 || material >= (int32_t)s->materials.size())
+        return b200pt_fail(B200PT_ERR_INVALID, "scene_bind_texture: material %d out of range", material);
+    if (slot < 0 || slot >= B200PT_TEX_SLOTS) return b200pt_fail(B200PT_ERR_INVALID, "scene_bind_texture: slot %d out of range", slot);
+    if (mipmap < 0 || mipmap >= (int32_t)s->mipmaps.size())
+        return b200pt_fail(B200PT_ERR_INVALID, "scene_bind_texture: mipmap %d out of range", mipmap);
+    const b200pt_material &m = s->materials[material];
+    bool ok;
+    switch (slot) {
+    case B200PT_TEX_KD: ok = m.type == B200PT_MAT_MATTE || m.type == B200PT_MAT_PLASTIC; break;
+    case B200PT_TEX_KS: ok = m.type == B200PT_MAT_PLASTIC || m.type == B200PT_MAT_GLASS; break;
+    case B200PT_TEX_KT: ok = m.type == B200PT_MAT_GLASS && m.variant != 2; break;
+    case B200PT_TEX_ETA:
+    case B200PT_TEX_K: ok = m.type == B200PT_MAT_METAL; break;
+    case B200PT_TEX_ROUGHNESS_U: ok = m.type == B200PT_MAT_PLASTIC || m.type == B200PT_MAT_METAL; break;
+    default: ok = m.type == B200PT_MAT_METAL; break;
+    }
+    if (!ok) return b200pt_fail(B200PT_ERR_INVALID, "scene_bind_texture: material %d (type %d, variant %d) has no slot %d", material, m.type, m.variant, slot);
+    const int want = slot >= B200PT_TEX_ROUGHNESS_U ? 1 : 3;
+    if (s->mipmap_channels[mipmap] != want)
+        return b200pt_fail(B200PT_ERR_INVALID, "scene_bind_texture: slot %d takes a %d-channel map, mipmap %d has %d", slot, want, mipmap,
+                           s->mipmap_channels[mipmap]);
+    if (s->tex_bind.empty()) {
+        DevTexBind none;
+        memset(&none, 0, sizeof(none));
+        none.mip = -1;
+        s->tex_bind.assign(s->materials.size() * B200PT_TEX_SLOTS, none);
+    }
+    DevTexBind &t = s->tex_bind[(size_t)material * B200PT_TEX_SLOTS + slot];
+    t.mip = mipmap;
+    t.su = su;
+    t.sv = sv;
+    t.du = du;
+    t.dv = dv;
+    t.remap = remap_roughness ? 1 : 0;
     return B200PT_OK;
 }
 
@@ -1272,6 +1384,15 @@ int b200pt_render_create(b200pt_scene *scene, const b200pt_camera_desc *cam, con
         ALLOC(d_med_spectra, med_spectra.size());
     }
     float *d_filter_table = nullptr;
+    // image textures: the MIPMaps and the binding table; the first hit rebuilds the camera ray from pFilm
+    const bool textured = !scene->tex_bind.empty();
+    DevMipmap *d_mipmaps = nullptr;
+    DevTexBind *d_tex_bind = nullptr;
+    if (textured) {
+        ALLOC(d_mipmaps, scene->mipmaps.size());
+        ALLOC(d_tex_bind, scene->tex_bind.size());
+        if (!filter_general) ALLOC(H.pfilm, cap);
+    }
     if (filter_general) {
         ALLOC(d_filter_table, 256);
         ALLOC(H.pfilm, cap);
@@ -1340,6 +1461,17 @@ int b200pt_render_create(b200pt_scene *scene, const b200pt_camera_desc *cam, con
     H.has_delta_lights = has_delta ? 1 : 0;
     H.infinite = d_infinite;
     H.n_infinite = (int)infinite.size();
+    H.mipmaps = d_mipmaps;
+    H.tex_bind = d_tex_bind;
+    if (textured) {
+        // PerspectiveCamera's constructor (perspective.cpp:55-58) and SamplerIntegrator::Render (integrator.cpp:285)
+        const V3 c0 = xform_point(cam->raster_to_camera, mk(0.f, 0.f, 0.f));
+        const V3 cx = xform_point(cam->raster_to_camera, mk(1.f, 0.f, 0.f)) - c0;
+        const V3 cy = xform_point(cam->raster_to_camera, mk(0.f, 1.f, 0.f)) - c0;
+        H.dx_camera[0] = cx.x, H.dx_camera[1] = cx.y, H.dx_camera[2] = cx.z;
+        H.dy_camera[0] = cy.x, H.dy_camera[1] = cy.y, H.dy_camera[2] = cy.z;
+        H.diff_scale = 1 / std::sqrt((float)smp->samples_per_pixel);
+    }
     H.light_cdf = d_cdf;
     H.light_func = d_func;
     cudaStream_t st = ctx->stream;
@@ -1359,6 +1491,10 @@ int b200pt_render_create(b200pt_scene *scene, const b200pt_camera_desc *cam, con
     if (!infinite.empty()) {
         CUDA_TRY(cudaMemcpyAsync(d_infinite, infinite.data(), infinite.size() * sizeof(DevInfinite), cudaMemcpyHostToDevice, st));
         CUDA_TRY(cudaStreamSynchronize(st));  // `infinite` is a local
+    }
+    if (textured) {
+        CUDA_TRY(cudaMemcpyAsync(d_mipmaps, scene->mipmaps.data(), scene->mipmaps.size() * sizeof(DevMipmap), cudaMemcpyHostToDevice, st));
+        CUDA_TRY(cudaMemcpyAsync(d_tex_bind, scene->tex_bind.data(), scene->tex_bind.size() * sizeof(DevTexBind), cudaMemcpyHostToDevice, st));
     }
     if (scene->nspec) {
         if (b200pt_s60::render_dev_size() != sizeof(RenderDev)) {
@@ -1548,7 +1684,7 @@ int b200pt_render_tiles(b200pt_render *r, const int32_t *tiles, int64_t n_tiles)
         CUDA_TRY(cudaMemsetAsync(H.pix_bleed, 0, (size_t)nb * 256, st));
         {
             LaunchTimer lt(r, st, 2);
-            LAUNCH_SPEC(launch_raygen, dev, (uint32_t)first, nb, n_slots, st);
+            LAUNCH_SPEC(launch_raygen, dev, (uint32_t)first, nb, n_slots, H.tex_bind != nullptr, st);
         }
         // Launch order per bounce b (path.cpp:81-188):
         //   closest(b) -> shade(b) -> { any(b), MIS-closest(b) } || closest(b+1) -> resolve(b) -> shade(b+1) ...
@@ -1568,7 +1704,7 @@ int b200pt_render_tiles(b200pt_render *r, const int32_t *tiles, int64_t n_tiles)
         const bool tl = two_level(r->scene) && !r->instrumented;  // instances inside the traversal kernel
         const bool has_spheres = H.scene.n_spheres > 0 || (H.scene.n_instances > 0 && !tl);  // "extra shapes" pass needed
         const bool full_shade = has_spheres || H.scene.n_instances > 0 || H.has_delta_lights || H.scene.tri_n != nullptr ||
-                                H.scene.tri_uv != nullptr || H.volpath || H.n_infinite > 0;
+                                H.scene.tri_uv != nullptr || H.volpath || H.n_infinite > 0 || H.tex_bind != nullptr;
         // escaped path rays of bounce b (scenes with infinite lights, RGB build only): after resolve(b - 1), before shade(b + 1)
         // rewrites the bounce's path queue
         auto escape = [&](int b) {

@@ -190,7 +190,9 @@ __device__ __forceinline__ bool pixel_rendered(const RenderDev *R, const TileRec
 }
 
 // ---------------------------------------------------------------------- raygen
-__global__ void __launch_bounds__(256) k_raygen(const RenderDev *R, uint32_t first_tile, uint32_t n_slots) {
+// PFILM: keep pFilm for every sample, not only under a general filter (textured scenes rebuild the camera ray's differentials)
+template <bool PFILM>
+__device__ __forceinline__ void raygen(const RenderDev *R, uint32_t first_tile, uint32_t n_slots) {
     const uint32_t slot = blockIdx.x * blockDim.x + threadIdx.x;
     bool valid = false;
     if (slot < n_slots) {
@@ -225,7 +227,7 @@ __global__ void __launch_bounds__(256) k_raygen(const RenderDev *R, uint32_t fir
             if ((int)ceilf(dy - 0.5f) < py) code |= 4u;
             if ((int)floorf(dy + 0.5f) + 1 > py + 1) code |= 8u;
             if (code) R->pix_bleed[tb * 256u + pix] = 1;
-            if (R->filter_general) R->pfilm[slot] = make_float2(pFilm[0], pFilm[1]);
+            if (PFILM || R->filter_general) R->pfilm[slot] = make_float2(pFilm[0], pFilm[1]);
             PathRec &P = R->path[slot];
             P.o = f4(o, 1.f);                                // etaScale = 1
             P.d = f4(d, __uint_as_float((uint32_t)st.dim));  // dim = 5, bounces = 0, flags = 0
@@ -241,6 +243,14 @@ __global__ void __launch_bounds__(256) k_raygen(const RenderDev *R, uint32_t fir
     const uint32_t pos = warp_append(&R->qcount[Q_PATH], valid);
     if (valid) R->q_path[0][pos] = slot;
 }
+__global__ void __launch_bounds__(256) k_raygen(const RenderDev *R, uint32_t first_tile, uint32_t n_slots) {
+    raygen<false>(R, first_tile, n_slots);
+}
+#if B200PT_NSPEC == 3
+__global__ void __launch_bounds__(256) k_raygen_pfilm(const RenderDev *R, uint32_t first_tile, uint32_t n_slots) {
+    raygen<true>(R, first_tile, n_slots);
+}
+#endif
 
 #if B200PT_NSPEC == 3  // spectrum-independent: compiled once, in the RGBSpectrum translation unit
 // ----------------------------------------------------------------------- trace
@@ -1082,21 +1092,165 @@ __device__ __forceinline__ DeltaLight delta_of(const DevLight &l, const Spec &in
 // ---- InfiniteAreaLight (lights/infinite.cpp:92-132) over the host's level-0 texels and Distribution2D tables
 #define PT_INV_PI ((float)0.31830988618379067154)
 #define PT_INV_2PI ((float)0.15915494309189533577)
-// MIPMap::triangle(0, st) (mipmap.h:262-273): bilinear, Repeat wrap (Mod, pbrt.h), the weights formed first
-__device__ __forceinline__ Spec infinite_lookup(const DevInfinite &L, float st0, float st1) {
-    const float s = st0 * L.w - 0.5f, t = st1 * L.h - 0.5f;
+// Mod (pbrt.h)
+__device__ __forceinline__ int pt_mod(int a, int b) {
+    const int r = a - (a / b) * b;
+    return r < 0 ? r + b : r;
+}
+// MIPMap::triangle(level, st) (mipmap.h:262-273) on a level of w x h texels: bilinear, the weights formed first;
+// texel(s, t) is MIPMap::Texel with the map's wrap mode
+template <class Texel>
+__device__ __forceinline__ Spec mip_bilerp(int w, int h, float st0, float st1, const Texel &texel) {
+    const float s = st0 * w - 0.5f, t = st1 * h - 0.5f;
     const int s0 = (int)floorf(s), t0 = (int)floorf(t);
     const float ds = s - s0, dt = t - t0;
-    auto mod = [](int a, int b) {
-        const int r = a - (a / b) * b;
-        return r < 0 ? r + b : r;
-    };
-    auto texel = [&](int si, int ti) {
-        const float4 v = L.texels[(size_t)mod(ti, L.h) * L.w + mod(si, L.w)];
-        return rgb(v.x, v.y, v.z);
-    };
     return (1 - ds) * (1 - dt) * texel(s0, t0) + (1 - ds) * dt * texel(s0, t0 + 1) + ds * (1 - dt) * texel(s0 + 1, t0) +
            ds * dt * texel(s0 + 1, t0 + 1);
+}
+// MIPMap::triangle(0, st) of the sky: Repeat wrap
+__device__ __forceinline__ Spec infinite_lookup(const DevInfinite &L, float st0, float st1) {
+    return mip_bilerp(L.w, L.h, st0, st1, [&](int si, int ti) {
+        const float4 v = L.texels[(size_t)pt_mod(ti, L.h) * L.w + pt_mod(si, L.w)];
+        return rgb(v.x, v.y, v.z);
+    });
+}
+
+// ---- ImageTexture lookups: MIPMap (mipmap.h:220-353) on RGB texels; a float map runs the same arithmetic on x
+// MIPMap::Texel (mipmap.h:220-242)
+__device__ __forceinline__ Spec mip_texel(const DevMipmap &M, int level, int s, int t) {
+    const int w = M.w[level], h = M.h[level];
+    if (M.wrap == B200PT_WRAP_REPEAT) {
+        s = pt_mod(s, w);
+        t = pt_mod(t, h);
+    } else if (M.wrap == B200PT_WRAP_CLAMP) {
+        s = pt_mini(pt_maxi(s, 0), w - 1);
+        t = pt_mini(pt_maxi(t, 0), h - 1);
+    } else if (s < 0 || s >= w || t < 0 || t >= h) {
+        return rgb1(0.f);
+    }
+    const float4 v = M.texels[level][(size_t)t * w + s];
+    return rgb(v.x, v.y, v.z);
+}
+__device__ __forceinline__ Spec mip_triangle(const DevMipmap &M, int level, float st0, float st1) {
+    level = pt_mini(pt_maxi(level, 0), M.levels - 1);
+    return mip_bilerp(M.w[level], M.h[level], st0, st1, [&](int si, int ti) { return mip_texel(M, level, si, ti); });
+}
+__device__ __forceinline__ float pt_log2f(float x) { return pt_logf(x) * 1.442695040888963387004650940071f; }  // Log2, pbrt.h
+__device__ __forceinline__ Spec mip_lerp(float t, const Spec &a, const Spec &b) { return (1 - t) * a + t * b; }
+// MIPMap::Lookup(st, width) (mipmap.h:244-261)
+__device__ __forceinline__ Spec mip_lookup_width(const DevMipmap &M, float st0, float st1, float width) {
+    const float level = M.levels - 1 + pt_log2f(pt_max(width, (float)1e-8));
+    if (level < 0) return mip_triangle(M, 0, st0, st1);
+    if (level >= M.levels - 1) return mip_texel(M, M.levels - 1, 0, 0);
+    const int iLevel = (int)floorf(level);
+    const float delta = level - iLevel;
+    return mip_lerp(delta, mip_triangle(M, iLevel, st0, st1), mip_triangle(M, iLevel + 1, st0, st1));
+}
+// MIPMap::EWA (mipmap.h:305-353)
+__device__ Spec mip_ewa(const DevMipmap &M, int level, float st0, float st1, float d00, float d01, float d10, float d11) {
+    if (level >= M.levels) return mip_texel(M, M.levels - 1, 0, 0);
+    const float w = (float)M.w[level], h = (float)M.h[level];
+    st0 = st0 * w - 0.5f;
+    st1 = st1 * h - 0.5f;
+    d00 *= w;
+    d01 *= h;
+    d10 *= w;
+    d11 *= h;
+    float A = d01 * d01 + d11 * d11 + 1;
+    float B = -2 * (d00 * d01 + d10 * d11);
+    float C = d00 * d00 + d10 * d10 + 1;
+    const float invF = 1 / (A * C - B * B * 0.25f);
+    A *= invF;
+    B *= invF;
+    C *= invF;
+    const float det = -B * B + 4 * A * C;
+    const float invDet = 1 / det;
+    const float uSqrt = sqrtf(det * C), vSqrt = sqrtf(A * det);
+    const int s0 = (int)ceilf(st0 - 2 * invDet * uSqrt);
+    const int s1 = (int)floorf(st0 + 2 * invDet * uSqrt);
+    const int t0 = (int)ceilf(st1 - 2 * invDet * vSqrt);
+    const int t1 = (int)floorf(st1 + 2 * invDet * vSqrt);
+    Spec sum = rgb1(0.f);
+    float sumWts = 0;
+    for (int it = t0; it <= t1; ++it) {
+        const float tt = it - st1;
+        for (int is = s0; is <= s1; ++is) {
+            const float ss = is - st0;
+            const float r2 = A * ss * ss + B * ss * tt + C * tt * tt;
+            if (r2 < 1) {
+                const int index = pt_mini((int)(r2 * 128), 128 - 1);
+                const float weight = M.weight_lut[index];
+                sum = sum + mip_texel(M, level, is, it) * weight;
+                sumWts += weight;
+            }
+        }
+    }
+    return sum / sumWts;
+}
+// MIPMap::Lookup(st, dst0, dst1) (mipmap.h:276-303)
+__device__ Spec mip_lookup(const DevMipmap &M, float st0, float st1, float d00, float d01, float d10, float d11) {
+    if (M.trilinear) {
+        const float width = pt_max(pt_max(pt_abs(d00), pt_abs(d01)), pt_max(pt_abs(d10), pt_abs(d11)));
+        return mip_lookup_width(M, st0, st1, 2 * width);
+    }
+    if (d00 * d00 + d01 * d01 < d10 * d10 + d11 * d11) {
+        float t = d00;
+        d00 = d10;
+        d10 = t;
+        t = d01;
+        d01 = d11;
+        d11 = t;
+    }
+    const float majorLength = sqrtf(d00 * d00 + d01 * d01);
+    float minorLength = sqrtf(d10 * d10 + d11 * d11);
+    if (minorLength * M.max_aniso < majorLength && minorLength > 0) {
+        const float scale = majorLength / (minorLength * M.max_aniso);
+        d10 *= scale;
+        d11 *= scale;
+        minorLength *= scale;
+    }
+    if (minorLength == 0) return mip_triangle(M, 0, st0, st1);
+    const float lod = pt_max((float)0, M.levels - (float)1 + pt_log2f(minorLength));
+    const int ilod = (int)floorf(lod);
+    return mip_lerp(lod - ilod, mip_ewa(M, ilod, st0, st1, d00, d01, d10, d11), mip_ewa(M, ilod + 1, st0, st1, d00, d01, d10, d11));
+}
+// ImageTexture::Evaluate (imagemap.h) through UVMapping2D::Map (texture.cpp:93-99)
+__device__ __forceinline__ Spec texture_eval(const RenderDev *R, const DevTexBind &t, const TexGeom &g) {
+    return mip_lookup(R->mipmaps[t.mip], t.su * g.u + t.du, t.sv * g.v + t.dv, t.su * g.dudx, t.sv * g.dvdx, t.su * g.dudy,
+                      t.sv * g.dvdy);
+}
+// TrowbridgeReitzDistribution::RoughnessToAlpha (microfacet.h:123-128)
+__device__ __forceinline__ float roughness_to_alpha(float roughness) {
+    roughness = pt_max(roughness, (float)1e-3);
+    const float x = pt_logf(roughness);
+    return 1.62142f + 0.819955f * x + 0.1734f * x * x + 0.0171201f * x * x * x + 0.000640711f * x * x * x * x;
+}
+// Spectrum::Clamp() (spectrum.h:256-262, low 0, high Infinity)
+__device__ __forceinline__ void clamp_rgb(const Spec &v, float out[3]) {
+    for (int c = 0; c < 3; ++c) out[c] = v.c[c] < 0.f ? 0.f : (v.c[c] > pt_inf() ? pt_inf() : v.c[c]);
+}
+// The material record of one hit: the material's textured parameters looked up, clamped and remapped like its
+// ComputeScatteringFunctions does (matte.cpp:50-62, plastic.cpp:50-70, metal.cpp:64-80, glass.cpp:50-64, mirror.cpp:48-56);
+// make_bsdf's black tests then decide the lobes per hit
+__device__ void textured_material(const RenderDev *R, uint32_t mi, const TexGeom &g, b200pt_material *m) {
+    const DevTexBind *tb = R->tex_bind + (size_t)mi * B200PT_TEX_SLOTS;
+    float *const spectra[5] = {m->kd, m->ks, m->kt, m->eta, m->k};
+    for (int slot = 0; slot < B200PT_TEX_SLOTS; ++slot) {
+        const DevTexBind t = tb[slot];
+        if (t.mip < 0) continue;
+        const Spec v = texture_eval(R, t, g);
+        if (slot <= B200PT_TEX_KT) {
+            clamp_rgb(v, spectra[slot]);
+        } else if (slot <= B200PT_TEX_K) {
+            for (int c = 0; c < 3; ++c) spectra[slot][c] = v.c[c];
+        } else {
+            const float a = t.remap ? roughness_to_alpha(v.c[0]) : v.c[0];
+            if (slot == B200PT_TEX_ROUGHNESS_U)
+                m->alpha_x = a;
+            else
+                m->alpha_y = a;
+        }
+    }
 }
 // SphericalPhi (geometry.h:1478-1481)
 __device__ __forceinline__ float spherical_phi(const V3 &v) {
@@ -1451,16 +1605,17 @@ __device__ __forceinline__ uint32_t pack_meta(int dim, int bounces, bool specula
 __device__ __forceinline__ uint32_t meta_with_dim(uint32_t meta, int dim) { return (meta & 0xffff0000u) | ((uint32_t)dim & 0xffffu); }
 
 // Re-derives the accepted closest hit P.hit of the path ray as a surface interaction: Shape::Intersect's values (t, b0,
-// b1, b2, or the sphere's root) do not depend on tMax.  Fills the hit's material word and light id too.
+// b1, b2, or the sphere's root) do not depend on tMax.  Fills the hit's material word and light id too, and with tg the
+// geometric dpdu / dpdv and uv a texture lookup needs.
 template <bool VTX>
 __device__ __forceinline__ bool accepted_hit(const RenderDev *R, const PathRec &P, const V3 &ro, const V3 &rd, Isect *is, uint32_t *mflags,
-                                             int *lightId) {
+                                             int *lightId, TexGeom *tg = nullptr) {
     const uint32_t ti = P.hit;
     bool found;
     if (VTX && is_sphere_hit(ti)) {
         const DevSphere *sp = R->scene.spheres + (ti & SPHERE_HIT_MASK);
         float th;
-        found = sphere_intersect(*sp, ro, rd, pt_inf(), &th, is);
+        found = sphere_intersect(*sp, ro, rd, pt_inf(), &th, is, tg);
         *mflags = sp->mat_flags;
         *lightId = sp->light_id;
     } else {
@@ -1481,7 +1636,8 @@ __device__ __forceinline__ bool accepted_hit(const RenderDev *R, const PathRec &
                 TriShading tsh;
                 load_shading<VTX>(R->scene, ti, *mflags, &tsh);
                 fill_isect(p0, p1, p2, (*mflags & B200PT_TRI_FLIP) != 0, tsh, h, d2, is);
-                instance_isect_to_world(*in, is);
+                if (tg) triangle_tex_geom(p0, p1, p2, tsh, h, tg);
+                instance_isect_to_world(*in, is, tg);
             }
         } else {
             found = triangle_test(p0, p1, p2, ro, make_shear(rd), pt_inf(), &h);
@@ -1489,6 +1645,7 @@ __device__ __forceinline__ bool accepted_hit(const RenderDev *R, const PathRec &
                 TriShading tsh;
                 load_shading<VTX>(R->scene, ti, *mflags, &tsh);
                 fill_isect(p0, p1, p2, (*mflags & B200PT_TRI_FLIP) != 0, tsh, h, rd, is);
+                if (tg) triangle_tex_geom(p0, p1, p2, tsh, h, tg);
             }
         }
     }
@@ -1596,6 +1753,34 @@ __device__ __forceinline__ void append_vertex_out(const RenderDev *R, uint32_t *
 }
 
 #if B200PT_NSPEC == 3
+// whether any parameter of material `mi` is an image texture (RenderDev::tex_bind != nullptr)
+__device__ __forceinline__ bool material_textured(const RenderDev *R, uint32_t mi) {
+    const DevTexBind *tb = R->tex_bind + (size_t)mi * B200PT_TEX_SLOTS;
+    bool any = false;
+    for (int k = 0; k < B200PT_TEX_SLOTS; ++k) any |= tb[k].mip >= 0;
+    return any;
+}
+// The uv derivatives of a textured hit.  Only camera rays carry differentials (every SpawnRay drops them, path.cpp:161,
+// volpath.cpp:115-121): at bounce 0 the camera ray is rebuilt from the sample's pFilm and lens sample (dimensions 3-4) and
+// counts as the path ray only if it is that ray bit for bit -- a ray that crossed a medium boundary was spawned anew.
+__device__ __forceinline__ void textured_hit(const RenderDev *R, const PathRec &P, uint32_t slot, const PathVertex &v, const Isect &is,
+                                             TexGeom *tg) {
+    bool has_diff = false;
+    V3 rdiff[4];
+    if (v.bounces == 0) {
+        const float2 pf = R->pfilm[slot];
+        const float pFilm[2] = {pf.x, pf.y};
+        SobolStream cs = sobol_stream(P.sobol, 3u);
+        float ul[2];
+        get2d(R->sampler, cs, ul);
+        V3 o, d;
+        float tMax;
+        generate_camera_ray(R->camera, pFilm, ul, &o, &d, &tMax);
+        has_diff = o.x == v.ro.x && o.y == v.ro.y && o.z == v.ro.z && d.x == v.rd.x && d.y == v.rd.y && d.z == v.rd.z;
+        if (has_diff) camera_ray_differentials(R->camera, R->dx_camera, R->dy_camera, R->diff_scale, pFilm, ul, o, d, rdiff);
+    }
+    compute_differentials(is, has_diff, rdiff, tg);
+}
 // resident CTAs per SM the shading kernels are compiled for (4 -> 128 registers; A/B builds: 5 -> 96, 6 -> 80)
 #ifndef B200PT_SHADE_MINCTAS
 #define B200PT_SHADE_MINCTAS 4
@@ -1622,7 +1807,9 @@ __global__ void __launch_bounds__(128, B200PT_SHADE_MINCTAS) k_shade(const Rende
             Isect is;
             uint32_t mflags;
             int lightId;
-            if (accepted_hit<VTX>(R, P, v.ro, v.rd, &is, &mflags, &lightId)) {
+            TexGeom tg;
+            const bool textures = VTX && R->tex_bind != nullptr;
+            if (accepted_hit<VTX>(R, P, v.ro, v.rd, &is, &mflags, &lightId, textures ? &tg : nullptr)) {
                 // path.cpp:91-101: emitted light at the first vertex or after a specular bounce
                 if (v.bounces == 0 || v.specularBounce) {
                     if (lightId >= 0) {
@@ -1634,7 +1821,15 @@ __global__ void __launch_bounds__(128, B200PT_SHADE_MINCTAS) k_shade(const Rende
                 if (v.bounces < R->max_depth) {  // path.cpp:104
                     Bsdf bsdf;
                     const uint32_t mi = mflags & 0xffffu;
-                    make_bsdf<MAT>(R->scene.materials[mi], R->scene.material_spectra + (size_t)mi * (5 * B200PT_NSPEC), is, &bsdf);
+                    const b200pt_material *mat = &R->scene.materials[mi];
+                    b200pt_material texMat;
+                    if (textures && material_textured(R, mi)) {
+                        texMat = *mat;
+                        textured_hit(R, P, slot, v, is, &tg);
+                        textured_material(R, mi, tg, &texMat);
+                        mat = &texMat;
+                    }
+                    make_bsdf<MAT>(*mat, R->scene.material_spectra + (size_t)mi * (5 * B200PT_NSPEC), is, &bsdf);
                     SobolStream st = sobol_stream(P.sobol, v.meta);
                     const SamplerParams &sp = R->sampler;
                     // path.cpp:119-128 -> UniformSampleOneLight (integrator.cpp:85-106)
@@ -2955,9 +3150,17 @@ __global__ void k_debug_camera(const RenderDev *R, int px, int py, int n, b200pt
 
 #endif  // B200PT_NSPEC == 3
 // -------------------------------------------------------------------- launchers
-void launch_raygen(const RenderDev *dev, uint32_t batch_first_tile, uint32_t n_batch_tiles, uint32_t n_slots,
+void launch_raygen(const RenderDev *dev, uint32_t batch_first_tile, uint32_t n_batch_tiles, uint32_t n_slots, bool keep_pfilm,
                    cudaStream_t s) {
     (void)n_batch_tiles;
+#if B200PT_NSPEC == 3
+    if (keep_pfilm) {
+        B200PT_LAUNCH(B200PT_KERNEL(k_raygen_pfilm), (n_slots + 255) / 256, 256, s, dev, batch_first_tile, n_slots);
+        return;
+    }
+#else
+    (void)keep_pfilm;
+#endif
     B200PT_LAUNCH(B200PT_KERNEL(k_raygen), (n_slots + 255) / 256, 256, s, dev, batch_first_tile, n_slots);
 }
 

@@ -47,6 +47,21 @@ struct DevInfinite {
     float two_world_radius;
 };
 
+// ImageTexture's MIPMap (b200pt_mipmap): every level as float4 texels (RGB, or the float value in x), MIPMap::weightLut
+struct DevMipmap {
+    int levels, wrap, trilinear;
+    float max_aniso;
+    int w[B200PT_MIPMAP_MAX_LEVELS], h[B200PT_MIPMAP_MAX_LEVELS];
+    const float4 *texels[B200PT_MIPMAP_MAX_LEVELS];
+    float weight_lut[128];
+};
+// A texture bound to one material parameter (b200pt_scene_bind_texture): mip < 0 = the material's constant
+struct DevTexBind {
+    int mip;
+    float su, sv, du, dv;  // UVMapping2D
+    int remap;             // roughness slots: RoughnessToAlpha after the lookup
+};
+
 struct DevScene {
     const U4 *nodes;
     const uint32_t *tri_base;  // per node: first triangle of its leaf children (wbvh.h)
@@ -202,6 +217,13 @@ struct RenderDev {
     // Scene::infiniteLights order; scenes with n_infinite > 0 run the full shading variant (RGB build only)
     const DevInfinite *infinite;
     int n_infinite;
+    // image textures (RGB build): tex_bind[material * B200PT_TEX_SLOTS + slot], nullptr = no textured material; textured
+    // scenes run the full shading variant, and k_raygen keeps every camera sample's pFilm so that the first hit can
+    // rebuild the camera ray's differentials
+    const DevMipmap *mipmaps;
+    const DevTexBind *tex_bind;
+    float diff_scale;          // 1 / sqrt(samplesPerPixel) (integrator.cpp:285)
+    float dx_camera[3], dy_camera[3];  // PerspectiveCamera::dxCamera / dyCamera (perspective.cpp:55-58)
 };
 
 // resident CTAs of k_trace per SM (128 threads each).  7 (up to 72 registers, no spills) measured fastest on the H100
@@ -254,7 +276,8 @@ __device__ __forceinline__ T &slot_out(T *base, uint32_t slot, int stride) {
     return *reinterpret_cast<T *>(reinterpret_cast<char *>(base) + (size_t)slot * (size_t)stride);
 }
 
-void launch_raygen(const RenderDev *dev, uint32_t batch_first_tile, uint32_t n_batch_tiles, uint32_t n_slots,
+// keep_pfilm: store every sample's pFilm (textured scenes) even with the box filter
+void launch_raygen(const RenderDev *dev, uint32_t batch_first_tile, uint32_t n_batch_tiles, uint32_t n_slots, bool keep_pfilm,
                    cudaStream_t s);
 // grid = SMs of the device (the launcher multiplies by B200PT_TRACE_CTAS)
 void launch_trace(const TraceArgs &a, bool any_hit, bool classify, bool count, int n_sm, cudaStream_t s);

@@ -436,8 +436,8 @@ B200_HD void concentric_sample_disk(const float u[2], float out[2]) {
 }
 
 // cameras/perspective.cpp:95-144 (main ray) + transform.h:251-264.  The ray
-// differentials only feed texture filtering (interaction.cpp:103-149), which
-// is dead for constant textures, so they are not generated.
+// differentials only feed image-texture filtering (interaction.cpp:103-149);
+// camera_ray_differentials rebuilds them where a textured hit needs them.
 B200_HD void generate_camera_ray(const CameraParams &cam, const float pFilm[2], const float uLens[2], V3 *o,
                                  V3 *d, float *tMax) {
     V3 pc = xform_point(cam.r2c, mk(pFilm[0], pFilm[1], 0.f));
@@ -465,6 +465,44 @@ B200_HD void generate_camera_ray(const CameraParams &cam, const float pFilm[2], 
     *o = wo;
     *d = wd;
     *tMax = tm;
+}
+
+// The differentials of the camera ray generate_camera_ray makes from the same sample: cameras/perspective.cpp:117-138 in
+// camera space (dxCamera / dyCamera as the constructor computes them, :55-58), CameraToWorld (transform.h:266-277, the
+// offset points without error bounds) and RayDifferential::ScaleDifferentials(scale) against the world-space main ray
+// (o, d) (geometry.h:946-951).  r[0..3] = rxOrigin, rxDirection, ryOrigin, ryDirection.
+B200_HD void camera_ray_differentials(const CameraParams &cam, const float dxCamera[3], const float dyCamera[3], float scale,
+                                      const float pFilm[2], const float uLens[2], const V3 &o, const V3 &d, V3 r[4]) {
+    const V3 pc = xform_point(cam.r2c, mk(pFilm[0], pFilm[1], 0.f));
+    const V3 dxc = mk(dxCamera[0], dxCamera[1], dxCamera[2]), dyc = mk(dyCamera[0], dyCamera[1], dyCamera[2]);
+    V3 rxo, rxd, ryo, ryd;
+    if (cam.lens_radius > 0.f) {
+        float dd[2];
+        concentric_sample_disk(uLens, dd);
+        const float lx = cam.lens_radius * dd[0], ly = cam.lens_radius * dd[1];
+        const V3 dx = normalize(pc + dxc);
+        float ft = cam.focal_distance / dx.z;
+        V3 pFocus = mk(0.f, 0.f, 0.f) + (ft * dx);
+        rxo = mk(lx, ly, 0.f);
+        rxd = normalize(pFocus - rxo);
+        const V3 dy = normalize(pc + dyc);
+        ft = cam.focal_distance / dy.z;
+        pFocus = mk(0.f, 0.f, 0.f) + (ft * dy);
+        ryo = mk(lx, ly, 0.f);
+        ryd = normalize(pFocus - ryo);
+    } else {
+        rxo = ryo = mk(0.f, 0.f, 0.f);
+        rxd = normalize(pc + dxc);
+        ryd = normalize(pc + dyc);
+    }
+    rxo = xform_point(cam.c2w, rxo);
+    ryo = xform_point(cam.c2w, ryo);
+    rxd = xform_vector(cam.c2w, rxd);
+    ryd = xform_vector(cam.c2w, ryd);
+    r[0] = o + (rxo - o) * scale;
+    r[1] = d + (rxd - d) * scale;
+    r[2] = o + (ryo - o) * scale;
+    r[3] = d + (ryd - d) * scale;
 }
 
 // ------------------------------------------------------------------- triangle
@@ -605,6 +643,52 @@ struct Isect {
     V3 ns;                // shading.n
     V3 sdpdu;             // shading.dpdu
 };
+// What texture lookups need of a surface hit besides Isect: the geometric SurfaceInteraction::dpdu / dpdv and uv (world
+// space, like the hit) and the screen-space uv derivatives ComputeDifferentials leaves
+struct TexGeom {
+    V3 dpdu, dpdv;
+    float u, v;
+    float dudx, dvdx, dudy, dvdy;
+};
+// SurfaceInteraction::ComputeDifferentials (interaction.cpp:103-149) for a ray with differentials r[0..3] = rxOrigin,
+// rxDirection, ryOrigin, ryDirection; has_diff == false (or a failed plane intersection) zeroes the derivatives
+B200_HD void compute_differentials(const Isect &is, bool has_diff, const V3 r[4], TexGeom *g) {
+    g->dudx = g->dvdx = g->dudy = g->dvdy = 0.f;
+    if (!has_diff) return;
+    const V3 n = is.n, p = is.p;
+    const float d = dot(n, p);
+    const float tx = -(dot(n, r[0]) - d) / dot(n, r[1]);
+    if (pt_isinf(tx) || tx != tx) return;
+    const V3 px = r[0] + tx * r[1];
+    const float ty = -(dot(n, r[2]) - d) / dot(n, r[3]);
+    if (pt_isinf(ty) || ty != ty) return;
+    const V3 py = r[2] + ty * r[3];
+    int d0, d1;
+    if (pt_abs(n.x) > pt_abs(n.y) && pt_abs(n.x) > pt_abs(n.z)) {
+        d0 = 1;
+        d1 = 2;
+    } else if (pt_abs(n.y) > pt_abs(n.z)) {
+        d0 = 0;
+        d1 = 2;
+    } else {
+        d0 = 0;
+        d1 = 1;
+    }
+    const float A00 = comp(g->dpdu, d0), A01 = comp(g->dpdv, d0), A10 = comp(g->dpdu, d1), A11 = comp(g->dpdv, d1);
+    // SolveLinearSystem2x2 (transform.cpp:41-49); a failed solve leaves its pair at 0
+    auto solve = [&](float b0, float b1, float *x0, float *x1) {
+        const float det = A00 * A11 - A01 * A10;
+        if (pt_abs(det) < 1e-10f) return;
+        const float y0 = (A11 * b0 - A01 * b1) / det;
+        const float y1 = (A00 * b1 - A10 * b0) / det;
+        if (y0 != y0 || y1 != y1) return;
+        *x0 = y0;
+        *x1 = y1;
+    };
+    solve(comp(px, d0) - comp(p, d0), comp(px, d1) - comp(p, d1), &g->dudx, &g->dvdx);
+    solve(comp(py, d0) - comp(p, d0), comp(py, d1) - comp(p, d1), &g->dudy, &g->dvdy);
+}
+
 B200_HD void fill_isect(const V3 &p0, const V3 &p1, const V3 &p2, bool flip, const TriShading &sh, const TriHit &h,
                         const V3 &rayD, Isect *is) {
     V3 dpdu, dpdv;
@@ -643,6 +727,13 @@ B200_HD void fill_isect(const V3 &p0, const V3 &p1, const V3 &p2, bool flip, con
         is->ns = n;
     }
     is->n = n;
+}
+
+// The triangle's SurfaceInteraction::dpdu / dpdv and uv (triangle.cpp:293-318, :329-330)
+B200_HD void triangle_tex_geom(const V3 &p0, const V3 &p1, const V3 &p2, const TriShading &sh, const TriHit &h, TexGeom *g) {
+    triangle_partials(p0, p1, p2, sh.uv, &g->dpdu, &g->dpdv);
+    g->u = h.b0 * sh.uv[0] + h.b1 * sh.uv[2] + h.b2 * sh.uv[4];
+    g->v = h.b0 * sh.uv[1] + h.b1 * sh.uv[3] + h.b2 * sh.uv[5];
 }
 
 // core/geometry.h:1440-1460

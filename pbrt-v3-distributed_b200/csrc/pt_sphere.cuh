@@ -299,8 +299,10 @@ B200_HD bool sphere_leaf_test(const DevSphere &sp, const V3 &ro, const V3 &rd, f
     return (tMin < rayTMax) && (tMax > 0);
 }
 
-// ---- Sphere::Intersect / IntersectP (sphere.cpp:49-212).  Returns false or *tHit (+ *is when is != nullptr).
-B200_HD bool sphere_intersect(const DevSphere &sp, const V3 &ro, const V3 &rd, float rayTMax, float *tHit, Isect *is) {
+// ---- Sphere::Intersect / IntersectP (sphere.cpp:49-212).  Returns false or *tHit (+ *is when is != nullptr, and the hit's
+// uv and world-space dpdu / dpdv, sphere.cpp:102-120, when tg != nullptr).
+B200_HD bool sphere_intersect(const DevSphere &sp, const V3 &ro, const V3 &rd, float rayTMax, float *tHit, Isect *is,
+                              TexGeom *tg = nullptr) {
     const float radius = sp.radius;
     V3 oErr, dErr;
     V3 o = xform_point_err(sp.w2o, ro, &oErr);
@@ -363,6 +365,14 @@ B200_HD bool sphere_intersect(const DevSphere &sp, const V3 &ro, const V3 &rd, f
     is->sdpdu = xform_vector(sp.o2w, dpdu);
     const V3 sn = normalize(xform_normal(sp.w2o, n));
     is->ns = (dot(sn, is->n) < 0.f) ? -sn : sn;
+    if (tg) {
+        float phi = pt_atan2f(pHit.y, pHit.x);
+        if (phi < 0) phi += 2 * PT_PI;
+        tg->u = phi / sp.phi_max;
+        tg->v = (theta - sp.theta_min) / (sp.theta_max - sp.theta_min);
+        tg->dpdu = xform_vector(sp.o2w, dpdu);
+        tg->dpdv = xform_vector(sp.o2w, dpdv);
+    }
     return true;
 }
 
@@ -480,9 +490,13 @@ B200_HD bool instance_leaf_test(const DevInstance &in, const V3 &ro, const V3 &r
     }
     return sphere_leaf_test(box, ro, rd, rayTMax);
 }
-// InstanceToWorld(SurfaceInteraction), transform.cpp:262-297
-B200_HD void instance_isect_to_world(const DevInstance &in, Isect *is) {
+// InstanceToWorld(SurfaceInteraction), transform.cpp:262-297 (tg: the texture lookup's dpdu / dpdv too)
+B200_HD void instance_isect_to_world(const DevInstance &in, Isect *is, TexGeom *tg = nullptr) {
     if (in.is_identity) return;
+    if (tg) {
+        tg->dpdu = xform_vector(in.i2w, tg->dpdu);
+        tg->dpdv = xform_vector(in.i2w, tg->dpdv);
+    }
     Isect w = *is;
     w.p = xform_point_err_in(in.i2w, is->p, is->pError, &w.pError);
     w.n = normalize(xform_normal(in.w2i, is->n));

@@ -84,6 +84,7 @@
 #include "shapes/sphere.h"
 #include "shapes/triangle.h"
 #include "textures/constant.h"
+#include "textures/imagemap.h"
 #undef private
 #undef protected
 
@@ -167,11 +168,79 @@ struct Flattened {
         float margFuncInt, lightToWorld[16], powerRGB[3];
     };
     std::vector<Infinite> infinite;
+    // ImageTextures (b200pt_scene_add_mipmap / b200pt_scene_bind_texture): every distinct MIPMap once (ImageTexture's
+    // cache shares one between textures with equal TexInfo), copied from the host's pyramid, and the bound slots
+    struct Mip {
+        int channels, wrap, trilinear;
+        float maxAniso, weightLut[128];
+        std::vector<int> w, h;
+        std::vector<std::vector<float>> levels;
+    };
+    std::vector<Mip> mipmaps;
+    std::unordered_map<const void *, int> mipOf;
+    struct Bind {
+        int material, slot, mip;
+        float su, sv, du, dv;
+        int remap;
+    };
+    std::vector<Bind> binds;
 };
 
-// materials/{matte,plastic,metal,glass}.cpp ComputeScatteringFunctions with constant textures
+// The MIPMap of an ImageTexture as the host built it (mipmap.h:116-218): the levels, the wrap mode, the filter settings
+// and weightLut, nothing recomputed
+template <typename Tm>
+int AddMipmap(const MIPMap<Tm> *mm, Flattened *f) {
+    auto it = f->mipOf.find(mm);
+    if (it != f->mipOf.end()) return it->second;
+    Flattened::Mip m;
+    m.channels = std::is_same<Tm, Float>::value ? 1 : 3;
+    m.wrap = mm->wrapMode == ImageWrap::Repeat ? B200PT_WRAP_REPEAT : mm->wrapMode == ImageWrap::Black ? B200PT_WRAP_BLACK : B200PT_WRAP_CLAMP;
+    m.trilinear = mm->doTrilinear ? 1 : 0;
+    m.maxAniso = mm->maxAnisotropy;
+    for (int i = 0; i < 128; ++i) m.weightLut[i] = MIPMap<Tm>::weightLut[i];
+    for (const auto &lv : mm->pyramid) {
+        m.w.push_back(lv->uSize());
+        m.h.push_back(lv->vSize());
+        std::vector<float> t;
+        t.reserve((size_t)lv->uSize() * lv->vSize() * m.channels);
+        for (int y = 0; y < lv->vSize(); ++y)
+            for (int x = 0; x < lv->uSize(); ++x) {
+                const Tm &v = (*lv)(x, y);
+                for (int c = 0; c < m.channels; ++c) t.push_back(((const Float *)&v)[c]);
+            }
+        m.levels.push_back(std::move(t));
+    }
+    const int id = (int)f->mipmaps.size();
+    f->mipmaps.push_back(std::move(m));
+    f->mipOf[mm] = id;
+    return id;
+}
+
+// A material parameter: a constant (*value) or, on RGBSpectrum hosts, an ImageTexture under UVMapping2D bound to
+// (material, slot) with the given remap flag
+template <typename T, typename Tm>
+bool TexturedParam(const std::shared_ptr<Texture<T>> &tex, T *value, int material, int slot, int remap, Flattened *f, std::string *why) {
+    if (ConstantValue(tex, value)) return true;
+    auto it = dynamic_cast<const ImageTexture<Tm, T> *>(tex.get());
+    if (!it) return *why = "textures other than \"constant\" and \"imagemap\"", false;
+    if (kSampledHost) return *why = "image textures in a SampledSpectrum build", false;
+    auto uv = dynamic_cast<const UVMapping2D *>(it->mapping.get());
+    if (!uv) return *why = "imagemap textures with a mapping other than \"uv\"", false;
+    *value = T(0.f);
+    f->binds.push_back({material, slot, AddMipmap(it->mipmap, f), uv->su, uv->sv, uv->du, uv->dv, remap});
+    return true;
+}
+bool SpectrumParam(const std::shared_ptr<Texture<Spectrum>> &tex, Spectrum *value, int material, int slot, Flattened *f, std::string *why) {
+    return TexturedParam<Spectrum, RGBSpectrum>(tex, value, material, slot, 0, f, why);
+}
+bool FloatParam(const std::shared_ptr<Texture<Float>> &tex, Float *value, int material, int slot, bool remap, Flattened *f, std::string *why) {
+    return TexturedParam<Float, Float>(tex, value, material, slot, remap ? 1 : 0, f, why);
+}
+
+// materials/{matte,plastic,metal,glass}.cpp ComputeScatteringFunctions with constant textures, or image textures the device
+// evaluates per hit (material index `mi`, bindings appended to f->binds; their constants here are 0 and ignored)
 // `rows`: the material's B200PT_MATERIAL_SPECTRA x 60 block (kd, ks, kt, eta, k), zero-initialised by the caller
-bool ConvertMaterial(const Material *m, b200pt_material *out, float *rows, std::string *why) {
+bool ConvertMaterial(const Material *m, b200pt_material *out, float *rows, int mi, Flattened *f, std::string *why) {
     memset(out, 0, sizeof(*out));
     float *rowKd = rows, *rowKs = rows + B200PT_SPECTRUM_SAMPLES, *rowKt = rows + 2 * B200PT_SPECTRUM_SAMPLES,
           *rowEta = rows + 3 * B200PT_SPECTRUM_SAMPLES, *rowK = rows + 4 * B200PT_SPECTRUM_SAMPLES;
@@ -179,7 +248,8 @@ bool ConvertMaterial(const Material *m, b200pt_material *out, float *rows, std::
     Float fv;
     if (auto mm = dynamic_cast<const MatteMaterial *>(m)) {
         if (mm->bumpMap) return *why = "bump maps", false;
-        if (!ConstantValue(mm->Kd, &sv) || !ConstantValue(mm->sigma, &fv)) return *why = "non-constant textures", false;
+        if (!SpectrumParam(mm->Kd, &sv, mi, B200PT_TEX_KD, f, why)) return false;
+        if (!ConstantValue(mm->sigma, &fv)) return *why = "a textured matte \"sigma\"", false;
         out->type = B200PT_MAT_MATTE;
         ToRGB(sv.Clamp(), out->kd, rowKd);
         if (Clamp(fv, 0, 90) != 0) {  // OrenNayar(r, sig), matte.cpp:59
@@ -191,8 +261,9 @@ bool ConvertMaterial(const Material *m, b200pt_material *out, float *rows, std::
     if (auto pm = dynamic_cast<const PlasticMaterial *>(m)) {
         if (pm->bumpMap) return *why = "bump maps", false;
         Spectrum kd, ks;
-        if (!ConstantValue(pm->Kd, &kd) || !ConstantValue(pm->Ks, &ks) || !ConstantValue(pm->roughness, &fv))
-            return *why = "non-constant textures", false;
+        if (!SpectrumParam(pm->Kd, &kd, mi, B200PT_TEX_KD, f, why) || !SpectrumParam(pm->Ks, &ks, mi, B200PT_TEX_KS, f, why) ||
+            !FloatParam(pm->roughness, &fv, mi, B200PT_TEX_ROUGHNESS_U, pm->remapRoughness, f, why))
+            return false;
         out->type = B200PT_MAT_PLASTIC;
         ToRGB(kd.Clamp(), out->kd, rowKd);
         ToRGB(ks.Clamp(), out->ks, rowKs);
@@ -205,10 +276,11 @@ bool ConvertMaterial(const Material *m, b200pt_material *out, float *rows, std::
         if (me->bumpMap) return *why = "bump maps", false;
         Spectrum eta, k;
         Float ur, vr;
-        if (!ConstantValue(me->eta, &eta) || !ConstantValue(me->k, &k)) return *why = "non-constant textures", false;
-        if (!ConstantValue(me->uRoughness ? me->uRoughness : me->roughness, &ur) ||
-            !ConstantValue(me->vRoughness ? me->vRoughness : me->roughness, &vr))
-            return *why = "non-constant textures", false;
+        if (!SpectrumParam(me->eta, &eta, mi, B200PT_TEX_ETA, f, why) || !SpectrumParam(me->k, &k, mi, B200PT_TEX_K, f, why))
+            return false;
+        if (!FloatParam(me->uRoughness ? me->uRoughness : me->roughness, &ur, mi, B200PT_TEX_ROUGHNESS_U, me->remapRoughness, f, why) ||
+            !FloatParam(me->vRoughness ? me->vRoughness : me->roughness, &vr, mi, B200PT_TEX_ROUGHNESS_V, me->remapRoughness, f, why))
+            return false;
         if (me->remapRoughness) {
             ur = TrowbridgeReitzDistribution::RoughnessToAlpha(ur);
             vr = TrowbridgeReitzDistribution::RoughnessToAlpha(vr);
@@ -224,9 +296,10 @@ bool ConvertMaterial(const Material *m, b200pt_material *out, float *rows, std::
         if (gm->bumpMap) return *why = "bump maps", false;
         Spectrum R, T;
         Float ur, vr, index;
-        if (!ConstantValue(gm->Kr, &R) || !ConstantValue(gm->Kt, &T) || !ConstantValue(gm->uRoughness, &ur) ||
-            !ConstantValue(gm->vRoughness, &vr) || !ConstantValue(gm->index, &index))
-            return *why = "non-constant textures", false;
+        if (!SpectrumParam(gm->Kr, &R, mi, B200PT_TEX_KS, f, why) || !SpectrumParam(gm->Kt, &T, mi, B200PT_TEX_KT, f, why)) return false;
+        if (!ConstantValue(gm->uRoughness, &ur) || !ConstantValue(gm->vRoughness, &vr))
+            return *why = "a textured glass roughness", false;
+        if (!ConstantValue(gm->index, &index)) return *why = "a textured glass \"index\"", false;
         out->type = B200PT_MAT_GLASS;
         ToRGB(R.Clamp(), out->ks, rowKs);
         ToRGB(T.Clamp(), out->kt, rowKt);
@@ -244,7 +317,7 @@ bool ConvertMaterial(const Material *m, b200pt_material *out, float *rows, std::
     }
     if (auto mr = dynamic_cast<const MirrorMaterial *>(m)) {
         if (mr->bumpMap) return *why = "bump maps", false;
-        if (!ConstantValue(mr->Kr, &sv)) return *why = "non-constant textures", false;
+        if (!SpectrumParam(mr->Kr, &sv, mi, B200PT_TEX_KS, f, why)) return false;
         out->type = B200PT_MAT_GLASS;  // the specular family; variant 2 = SpecularReflection(Kr, FresnelNoOp), mirror.cpp:45-56
         out->variant = 2;
         ToRGB(sv.Clamp(), out->ks, rowKs);
@@ -276,7 +349,7 @@ bool FlattenScene(const Scene &scene, Flattened *f, std::string *why, bool volum
         if (it == matIndex.end()) {
             b200pt_material bm;
             std::vector<float> rows((size_t)B200PT_MATERIAL_SPECTRA * B200PT_SPECTRUM_SAMPLES, 0.f);
-            if (!ConvertMaterial(m, &bm, rows.data(), why)) return false;
+            if (!ConvertMaterial(m, &bm, rows.data(), (int)f->materials.size(), f, why)) return false;
             it = matIndex.emplace(m, (int)f->materials.size()).first;
             f->materials.push_back(bm);
             if (kSampledHost) f->materialSpectra.insert(f->materialSpectra.end(), rows.begin(), rows.end());
@@ -744,6 +817,29 @@ class GpuIntegrator : public Base {
                     fwrite(&in.margFuncInt, 4, 1, df);
                     fwrite(in.powerRGB, 4, 3, df);
                 }
+                // image textures (appended after the infinite lights, behind a negative marker): the MIPMaps, then the bindings
+                if (!flat.binds.empty()) {
+                    const int32_t th[3] = {-2, (int32_t)flat.mipmaps.size(), (int32_t)flat.binds.size()};
+                    fwrite(th, 4, 3, df);
+                    for (const auto &m : flat.mipmaps) {
+                        const int32_t mh[4] = {(int32_t)m.levels.size(), m.channels, m.wrap, m.trilinear};
+                        fwrite(mh, 4, 4, df);
+                        fwrite(&m.maxAniso, 4, 1, df);
+                        fwrite(m.weightLut, 4, 128, df);
+                        for (size_t l = 0; l < m.levels.size(); ++l) {
+                            const int32_t wh[2] = {m.w[l], m.h[l]};
+                            fwrite(wh, 4, 2, df);
+                            fwrite(m.levels[l].data(), 4, m.levels[l].size(), df);
+                        }
+                    }
+                    for (const auto &b : flat.binds) {
+                        const int32_t bi[3] = {b.material, b.slot, b.mip};
+                        const float bf[4] = {b.su, b.sv, b.du, b.dv};
+                        fwrite(bi, 4, 3, df);
+                        fwrite(bf, 4, 4, df);
+                        fwrite(&b.remap, 4, 1, df);
+                    }
+                }
                 fclose(df);
             }
         }
@@ -788,6 +884,28 @@ class GpuIntegrator : public Base {
             memcpy(il.power_rgb, in.powerRGB, sizeof(il.power_rgb));
             B200_CHECK(b200pt_scene_set_infinite_light(gscene, in.light, &il));
         }
+        std::vector<int32_t> mipIds;
+        for (const auto &m : flat.mipmaps) {
+            b200pt_mipmap bm;
+            memset(&bm, 0, sizeof(bm));
+            if (m.levels.size() > B200PT_MIPMAP_MAX_LEVELS) return Error("gpupath: image textures larger than %d texels on a side are not supported", 1 << (B200PT_MIPMAP_MAX_LEVELS - 1));
+            bm.n_levels = (int32_t)m.levels.size();
+            bm.channels = m.channels;
+            for (size_t l = 0; l < m.levels.size(); ++l) {
+                bm.width[l] = m.w[l];
+                bm.height[l] = m.h[l];
+                bm.texels[l] = m.levels[l].data();
+            }
+            bm.wrap = m.wrap;
+            bm.trilinear = m.trilinear;
+            bm.max_anisotropy = m.maxAniso;
+            memcpy(bm.weight_lut, m.weightLut, sizeof(bm.weight_lut));
+            int32_t mid = -1;
+            B200_CHECK(b200pt_scene_add_mipmap(gscene, &bm, &mid));
+            mipIds.push_back(mid);
+        }
+        for (const auto &b : flat.binds)
+            B200_CHECK(b200pt_scene_bind_texture(gscene, b.material, b.slot, mipIds[b.mip], b.su, b.sv, b.du, b.dv, b.remap));
         B200_CHECK(b200pt_render_create(gscene, &cd, &fd, &smpd, &id, &render));
         B200_CHECK(b200pt_ctx_synchronize(ctx));
         const auto t2 = now();

@@ -12,6 +12,7 @@ The same description can be written out as `.pbrt` + binary PLY
 """
 import ctypes as C
 import os
+import re
 import struct
 
 import numpy as np
@@ -139,7 +140,7 @@ class SceneArrays:
 
     def __init__(self, n_tris, materials=("matte",), soup_version=1, seed=1234, light_L=40.0,
                  n_lights=None, two_sided=False, reverse_orientation=(), shading_normals=(), uvs=(), spheres=(),
-                 objects=(), instances=(), delta_lights=(), infinite_lights=()):
+                 objects=(), instances=(), delta_lights=(), infinite_lights=(), textures=None):
         """spheres: dicts {center, radius, material (a name in `materials` or "black"), emit (radiance or
         None), scale (sx, sy, sz) or None, reverse_orientation} -- written as `Translate` + `Scale` +
         `Shape "sphere"` by write_pbrt, after the meshes."""
@@ -221,6 +222,11 @@ class SceneArrays:
         # infinite lights: dicts {L (rgb or scalar), scale (rgb or scalar), map (array [h][w][3], written as <name>_sky<k>.pfm
         # and named by "string mapname") or None, steps: [(op, args)] of the light's transform}; they follow the delta lights
         self.infinite_specs = [dict(x) for x in infinite_lights]
+        # image textures: {material name: {pbrt parameter ("Kd", "roughness", ...): texture spec, "params": extra material
+        # parameters}} with texture spec {map: [h][w][3] texels (written as a PFM), wrap, trilinear, maxanisotropy, scale,
+        # gamma, uscale, vscale, udelta, vdelta}; write_pbrt declares them as imagemap textures under the "uv" mapping.  The
+        # descriptors here keep the materials' constants: the texture tables come from the host (read_dump_textures)
+        self.texture_specs = {k: dict(v) for k, v in (textures or {}).items()}
         self._lights = (abi.AreaLight * max(nl + len(self.delta_specs) + len(self.infinite_specs) + n_sl, 1))()
         for i in range(nl):
             self._lights[i].triangle = i
@@ -442,6 +448,33 @@ def write_ply(path, tris, normals=None, uvs=None):
         f.write(rec.tobytes())
 
 
+TEXTURE_FLOAT_PARAMS = ("roughness", "uroughness", "vroughness")
+
+
+def _texture_lines(scene, name, dirname):
+    """The Texture statements of scene.texture_specs (and their PFMs); {material: material statement} for textured ones."""
+    lines, mats = [], {}
+    for mat, params in sorted(getattr(scene, "texture_specs", {}).items()):
+        stmt = PBRT_MATERIAL[mat]
+        for param, t in sorted((k, v) for k, v in params.items() if k != "params"):
+            tex = "%s_%s" % (mat, param)
+            pfm = "%s_tex_%s.pfm" % (name, tex)
+            write_pfm(os.path.join(dirname, pfm), np.asarray(t["map"], np.float32))
+            line = 'Texture "%s" "%s" "imagemap" "string filename" "%s"' % (tex, "float" if param in TEXTURE_FLOAT_PARAMS else "spectrum", pfm)
+            for key, kind in (("wrap", "string"), ("trilinear", "bool"), ("maxanisotropy", "float"), ("scale", "float"),
+                              ("gamma", "bool"), ("uscale", "float"), ("vscale", "float"), ("udelta", "float"), ("vdelta", "float")):
+                if key in t:
+                    v = t[key]
+                    line += ' "%s %s" [%s]' % (kind, key, ('"%s"' % v) if kind == "string" else
+                                               ('"true"' if v else '"false"') if kind == "bool" else "%.9g" % v)
+            lines.append(line)
+            stmt = re.sub(r' "\w+ %s" \[[^\]]*\]' % param, "", stmt) + ' "texture %s" "%s"' % (param, tex)
+        if params.get("params"):
+            stmt += " " + params["params"]
+        mats[mat] = stmt
+    return lines, mats
+
+
 def write_pbrt(dirname, name, scene, xres, yres, spp, max_depth=5, strategy="uniform", pixel_bounds=None,
                eye=(0, 0, -4.5), look=(0, 0, 0), up=(0, 1, 0), fov=35.0, lens_radius=0.0, focal_distance=1e6,
                crop_window=None, film_scale=1.0, max_sample_luminance=None, sampler="sobol", pixel_filter=None,
@@ -474,6 +507,9 @@ def write_pbrt(dirname, name, scene, xres, yres, spp, max_depth=5, strategy="uni
     lines += [integ, "WorldBegin"]
     if medium:
         lines.append('MediumInterface "fog" "fog"')
+    tex_lines, tex_mats = _texture_lines(scene, name, dirname)
+    lines += tex_lines
+    material = lambda m: tex_mats.get(m, PBRT_MATERIAL[m])
     for q in scene.light_quads:
         # quad() stores (p0 p1 p2)(p0 p2 p3); recover the 4 corners
         pts = [q[0][0], q[0][1], q[0][2], q[1][2]]
@@ -517,13 +553,13 @@ def write_pbrt(dirname, name, scene, xres, yres, spp, max_depth=5, strategy="uni
                   scene.uvs[sel] if m in scene.uv_meshes else None)
         if m in scene.reverse_orientation:
             lines += ["AttributeBegin", "ReverseOrientation"]
-        lines += [PBRT_MATERIAL[scene.material_names[m]], 'Shape "plymesh" "string filename" "%s"' % ply]
+        lines += [material(scene.material_names[m]), 'Shape "plymesh" "string filename" "%s"' % ply]
         if m in scene.reverse_orientation:
             lines += ["AttributeEnd"]
     for k, (o, part) in enumerate(zip(getattr(scene, "object_specs", ()), getattr(scene, "object_parts", ()))):
         ply = "%s_obj%d.ply" % (name, k)
         write_ply(os.path.join(dirname, ply), part)
-        lines += ['ObjectBegin "obj%d"' % k, "  " + PBRT_MATERIAL[o.get("material", "matte")],
+        lines += ['ObjectBegin "obj%d"' % k, "  " + material(o.get("material", "matte")),
                   '  Shape "plymesh" "string filename" "%s"' % ply, "ObjectEnd"]
     for ins in getattr(scene, "instance_specs", ()):
         lines.append("AttributeBegin")
@@ -541,7 +577,7 @@ def write_pbrt(dirname, name, scene, xres, yres, spp, max_depth=5, strategy="uni
                       '[%.9g %.9g %.9g] "float g" [%.9g] "float scale" [1]' % ((len(lines),) + tuple(b["sigma_a"]) + tuple(b["sigma_s"]) + (b.get("g", 0.0),)),
                       '  MediumInterface "cloud%d" "%s"' % (len(lines), "fog" if medium else ""), '  Material ""']
         else:
-            lines.append("  " + ('Material "matte" "rgb Kd" [0 0 0]' if mat == "black" else PBRT_MATERIAL[mat]))
+            lines.append("  " + ('Material "matte" "rgb Kd" [0 0 0]' if mat == "black" else material(mat)))
         lines.append("  Translate %.9g %.9g %.9g" % tuple(sp["center"]))
         if sp.get("scale"):
             lines.append("  Scale %.9g %.9g %.9g" % tuple(sp["scale"]))
@@ -560,6 +596,20 @@ def write_pbrt(dirname, name, scene, xres, yres, spp, max_depth=5, strategy="uni
 def read_dump_infinite(path, abi):
     """{light index: tables for Scene.set_infinite_light} of the InfiniteAreaLights an RGBSpectrum host wrote to its
     B200PT_DUMP_SCENE file (host/gpupath.cpp appends them after the descriptors)."""
+    return _read_dump_tail(path, abi)[0]
+
+
+def read_dump_textures(path, abi):
+    """(mipmaps, binds) of the image textures an RGBSpectrum host wrote to its B200PT_DUMP_SCENE file (behind the infinite
+    lights' tables): mipmaps are dicts {levels ([h][w][3] or [h][w] arrays), wrap, trilinear, max_anisotropy, weight_lut}
+    for Scene.add_mipmap, binds are dicts {material, slot, mipmap, su, sv, du, dv, remap} in the host's material order."""
+    return _read_dump_tail(path, abi)[1]
+
+
+TEXTURE_MARKER = -2  # host/gpupath.cpp: the image textures' tables follow the infinite lights' behind this int32
+
+
+def _read_dump_tail(path, abi):
     raw = open(path, "rb").read()
     hdr = np.frombuffer(raw, np.int64, 8)
     nt, nm, nl, nsph, has_n, has_uv = (int(x) for x in hdr[1:7])
@@ -576,15 +626,36 @@ def read_dump_infinite(path, abi):
         a = np.frombuffer(raw, np.float32, n, off).copy()
         off += 4 * n
         return a.reshape(shape) if shape else a
-    while off < len(raw):
-        light, w, h, nu, nv = (int(x) for x in np.frombuffer(raw, np.int32, 5, off))
-        off += 20
+
+    def ints(n):
+        nonlocal off
+        a = [int(x) for x in np.frombuffer(raw, np.int32, n, off)]
+        off += 4 * n
+        return a
+    while off < len(raw) and int(np.frombuffer(raw, np.int32, 1, off)[0]) != TEXTURE_MARKER:
+        light, w, h, nu, nv = ints(5)
         out[light] = dict(texels=take(w * h * 3, (h, w, 3)), light_to_world=take(16), cond_func=take(nv * nu, (nv, nu)),
                           cond_cdf=take(nv * (nu + 1), (nv, nu + 1)), cond_func_int=take(nv), marg_func=take(nv),
                           marg_cdf=take(nv + 1), marg_func_int=take(1)[0], power_rgb=take(3))
+    mips, binds = [], []
+    if off < len(raw):
+        _, nmip, nbind = ints(3)
+        for _ in range(nmip):
+            nlev, ch, wrap, tri = ints(4)
+            aniso = float(take(1)[0])
+            lut = take(128)
+            levels = []
+            for _ in range(nlev):
+                w, h = ints(2)
+                levels.append(take(w * h * ch, (h, w, 3) if ch == 3 else (h, w)))
+            mips.append(dict(levels=levels, wrap=wrap, trilinear=tri, max_anisotropy=aniso, weight_lut=lut))
+        for _ in range(nbind):
+            mat, slot, mip = ints(3)
+            su, sv, du, dv = (float(x) for x in take(4))
+            binds.append(dict(material=mat, slot=slot, mipmap=mip, su=su, sv=sv, du=du, dv=dv, remap=ints(1)[0]))
     if off != len(raw):
-        raise ValueError("%s: truncated infinite-light tables" % path)
-    return out
+        raise ValueError("%s: truncated infinite-light or texture tables" % path)
+    return out, (mips, binds)
 
 
 def read_pfm(path):
