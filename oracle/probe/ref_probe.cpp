@@ -17,6 +17,13 @@
 //   camrays <camera args> spp px py n             GetCameraSample + GenerateRayDifferential main rays
 //   intersect <tris.f32> <rays.bin> <out.bin>     BVHAccel (SAH, maxnodeprims 4) Intersect + IntersectP
 //   consts                                        default copper eta/k RGB, RoughnessToAlpha samples
+//   mipmap <req.bin> <out.bin>                    MIPMap<RGBSpectrum | Float> built from the request's texels: the
+//                                                 pyramid, weightLut, Lookup(st, dst0, dst1) and Lookup(st, width)
+//   infinite <map.pfm> <req.bin> <out.bin>        InfiniteAreaLight: level 0 of Lmap, the Distribution2D tables, both
+//                                                 matrices, Sample_Li, Pdf_Li and Le answers
+//   differentials <req.bin> <out.bin>             SurfaceInteraction::ComputeDifferentials: dudx dvdx dudy dvdy
+//   roughness <lo> <hi>                           RoughnessToAlpha of the floats with bits [lo, hi), raw to stdout
+// The request and answer layouts are those of tests/texlookup.py.
 // standard headers first: the access hack below must not reach them
 #include <algorithm>
 #include <atomic>
@@ -44,7 +51,9 @@
 #include "core/film.h"
 #include "core/interaction.h"
 #include "core/lowdiscrepancy.h"
+#include "core/light.h"
 #include "core/microfacet.h"
+#include "core/mipmap.h"
 #include "core/paramset.h"
 #include "core/primitive.h"
 #include "core/sampler.h"
@@ -56,6 +65,7 @@
 #include "filters/sinc.h"
 #include "filters/mitchell.h"
 #include "filters/gaussian.h"
+#include "lights/infinite.h"
 #include "materials/matte.h"
 #include "materials/metal.h"
 #include "samplers/halton.h"
@@ -88,6 +98,82 @@ static std::vector<float> readFloats(const char *fn) {
     if (fread(v.data(), 4, v.size(), f) != v.size()) die("short read");
     fclose(f);
     return v;
+}
+
+static std::vector<char> readBytes(const char *fn) {
+    FILE *f = fopen(fn, "rb");
+    if (!f) die("cannot open input");
+    fseek(f, 0, SEEK_END);
+    long n = ftell(f);
+    fseek(f, 0, SEEK_SET);
+    std::vector<char> v(n);
+    if (n && fread(v.data(), 1, n, f) != (size_t)n) die("short read");
+    fclose(f);
+    return v;
+}
+
+// Reads a request field by field
+struct Req {
+    std::vector<char> b;
+    size_t at = 0;
+    template <class T>
+    const T *take(size_t n) {
+        if (at + n * sizeof(T) > b.size()) die("request too short");
+        const T *p = (const T *)(b.data() + at);
+        at += n * sizeof(T);
+        return p;
+    }
+};
+
+static void put(FILE *f, const void *p, size_t bytes) {
+    if (bytes && fwrite(p, 1, bytes, f) != bytes) die("short write");
+}
+
+// Runs fn(i) for i in [0, n) on all cores (the reference's lookups are const)
+static void parallelRange(size_t n, const std::function<void(size_t)> &fn) {
+    const unsigned nt = std::max(1u, std::min(64u, std::thread::hardware_concurrency()));
+    std::vector<std::thread> pool;
+    const size_t per = (n + nt - 1) / nt;
+    for (unsigned t = 0; t < nt; ++t) {
+        const size_t lo = std::min(n, t * per), hi = std::min(n, lo + per);
+        pool.emplace_back([=, &fn]() {
+            for (size_t i = lo; i < hi; ++i) fn(i);
+        });
+    }
+    for (auto &th : pool) th.join();
+}
+
+// mipmap: request int32 {channels, w, h, wrap (ImageWrap), doTrilinear, nEwa, nWidth, 0}, float maxAnisotropy, texels
+// [h][w][channels], nEwa x {s, t, dst0.x, dst0.y, dst1.x, dst1.y}, nWidth x {s, t, width}.  Answer int32 {levels},
+// int32 {uSize, vSize} per level, every level's texels [v][u][channels], weightLut[128], the answers (channels floats
+// each).
+template <typename T>
+static void probeMipmap(Req &q, const int32_t *hdr, FILE *out) {
+    const int ch = hdr[0], w = hdr[1], h = hdr[2], nEwa = hdr[5], nWidth = hdr[6];
+    const float maxAniso = *q.take<float>(1);
+    const float *tex = q.take<float>((size_t)w * h * ch);
+    std::vector<T> img((size_t)w * h);
+    for (size_t i = 0; i < img.size(); ++i) memcpy((void *)&img[i], tex + i * ch, sizeof(float) * ch);
+    const float *ewa = q.take<float>((size_t)nEwa * 6), *wid = q.take<float>((size_t)nWidth * 3);
+    MIPMap<T> mm(Point2i(w, h), img.data(), hdr[4] != 0, maxAniso, (ImageWrap)hdr[3]);
+    const int32_t levels = mm.Levels();
+    put(out, &levels, 4);
+    for (const auto &lv : mm.pyramid) {
+        const int32_t wh[2] = {lv->uSize(), lv->vSize()};
+        put(out, wh, 8);
+    }
+    for (const auto &lv : mm.pyramid)
+        for (int t = 0; t < lv->vSize(); ++t)
+            for (int s = 0; s < lv->uSize(); ++s) put(out, &(*lv)(s, t), sizeof(float) * ch);
+    put(out, MIPMap<T>::weightLut, sizeof(float) * 128);
+    std::vector<T> a(nEwa), b(nWidth);
+    parallelRange(nEwa, [&](size_t i) {
+        const float *e = ewa + 6 * i;
+        a[i] = mm.Lookup(Point2f(e[0], e[1]), Vector2f(e[2], e[3]), Vector2f(e[4], e[5]));
+    });
+    parallelRange(nWidth, [&](size_t i) { b[i] = mm.Lookup(Point2f(wid[3 * i], wid[3 * i + 1]), wid[3 * i + 2]); });
+    for (const T &v : a) put(out, &v, sizeof(float) * ch);
+    for (const T &v : b) put(out, &v, sizeof(float) * ch);
 }
 
 struct Cam {
@@ -333,6 +419,119 @@ int main(int argc, char **argv) {
         for (float r : rough)
             printf("roughness_to_alpha %a %a\n", (double)r,
                    (double)TrowbridgeReitzDistribution::RoughnessToAlpha(r));
+    } else if (cmd == "mipmap") {
+        if (argc != 4) die("usage: mipmap <req.bin> <out.bin>");
+        Req q;
+        q.b = readBytes(argv[2]);
+        const int32_t *hdr = q.take<int32_t>(8);
+        if ((hdr[0] != 1 && hdr[0] != 3) || hdr[1] < 1 || hdr[2] < 1 || hdr[3] < 0 || hdr[3] > 2) die("bad mipmap request");
+        FILE *out = fopen(argv[3], "wb");
+        if (!out) die("cannot open output");
+        if (hdr[0] == 3)
+            probeMipmap<RGBSpectrum>(q, hdr, out);
+        else
+            probeMipmap<Float>(q, hdr, out);
+        fclose(out);
+    } else if (cmd == "infinite") {
+        // request: int32 {nSample, nPdf, nLe, nu, nv, 0}, float LightToWorld[16] (row major), worldRadius, ref.p[3], with nu > 0
+        // an image [nv][nu] whose Distribution2D replaces the light's (sizes no map gives: the map's are powers of two),
+        // nSample x u[2], nPdf x w[3], nLe x ray.d[3].  Answer: int32 {width, height, nu, nv}; level 0 of Lmap [height][width][3], every
+        // pConditionalV row's func, then cdf, then funcInt; pMarginal's func, cdf, funcInt; LightToWorld.m, WorldToLight.m;
+        // nSample x {wi[3], pdf, Li[3], P1().p[3]}, nPdf x Pdf_Li, nLe x Le[3]
+        if (argc != 5) die("usage: infinite <map.pfm> <req.bin> <out.bin>");
+        Req q;
+        q.b = readBytes(argv[3]);
+        const int32_t *hdr = q.take<int32_t>(6);
+        const float *m = q.take<float>(16), worldRadius = *q.take<float>(1), *rp = q.take<float>(3);
+        const float *img = hdr[3] > 0 ? q.take<float>((size_t)hdr[3] * hdr[4]) : nullptr;
+        const float *us = q.take<float>((size_t)hdr[0] * 2), *ws = q.take<float>((size_t)hdr[1] * 3),
+                    *ds = q.take<float>((size_t)hdr[2] * 3);
+        Matrix4x4 mat(m[0], m[1], m[2], m[3], m[4], m[5], m[6], m[7], m[8], m[9], m[10], m[11], m[12], m[13], m[14], m[15]);
+        InfiniteAreaLight light(Transform(mat), Spectrum(1.f), 1, argv[2]);
+        light.worldRadius = worldRadius;
+        if (img) light.distribution.reset(new Distribution2D(img, hdr[3], hdr[4]));
+        FILE *out = fopen(argv[4], "wb");
+        if (!out) die("cannot open output");
+        const auto &lv0 = *light.Lmap->pyramid[0];
+        const Distribution2D &d2 = *light.distribution;
+        const int32_t dims[4] = {lv0.uSize(), lv0.vSize(), d2.pConditionalV[0]->Count(), (int32_t)d2.pConditionalV.size()};
+        put(out, dims, 16);
+        for (int t = 0; t < lv0.vSize(); ++t)
+            for (int s = 0; s < lv0.uSize(); ++s) put(out, &lv0(s, t), 12);
+        for (const auto &row : d2.pConditionalV) put(out, row->func.data(), 4 * row->func.size());
+        for (const auto &row : d2.pConditionalV) put(out, row->cdf.data(), 4 * row->cdf.size());
+        for (const auto &row : d2.pConditionalV) put(out, &row->funcInt, 4);
+        put(out, d2.pMarginal->func.data(), 4 * d2.pMarginal->func.size());
+        put(out, d2.pMarginal->cdf.data(), 4 * d2.pMarginal->cdf.size());
+        put(out, &d2.pMarginal->funcInt, 4);
+        put(out, light.LightToWorld.m.m, 64);
+        put(out, light.WorldToLight.m.m, 64);
+        Interaction ref;
+        ref.p = Point3f(rp[0], rp[1], rp[2]);
+        std::vector<float> sa((size_t)hdr[0] * 10), pa(hdr[1]), la((size_t)hdr[2] * 3);
+        parallelRange(hdr[0], [&](size_t i) {
+            Vector3f wi(0, 0, 0);
+            Float pdf = 0;
+            VisibilityTester vis;
+            const Spectrum li = light.Sample_Li(ref, Point2f(us[2 * i], us[2 * i + 1]), &wi, &pdf, &vis);
+            const float o[10] = {wi.x, wi.y, wi.z, pdf, li[0], li[1], li[2], vis.p1.p.x, vis.p1.p.y, vis.p1.p.z};
+            memcpy(&sa[10 * i], o, sizeof(o));
+        });
+        parallelRange(hdr[1], [&](size_t i) { pa[i] = light.Pdf_Li(ref, Vector3f(ws[3 * i], ws[3 * i + 1], ws[3 * i + 2])); });
+        parallelRange(hdr[2], [&](size_t i) {
+            RayDifferential ray(Point3f(0, 0, 0), Vector3f(ds[3 * i], ds[3 * i + 1], ds[3 * i + 2]));
+            const Spectrum le = light.Le(ray);
+            for (int c = 0; c < 3; ++c) la[3 * i + c] = le[c];
+        });
+        put(out, sa.data(), 4 * sa.size());
+        put(out, pa.data(), 4 * pa.size());
+        put(out, la.data(), 4 * la.size());
+        fclose(out);
+    } else if (cmd == "differentials") {
+        // request: n x {p, n, dpdu, dpdv, rxOrigin, rxDirection, ryOrigin, ryDirection} (24 floats); answer n x {dudx, dvdx,
+        // dudy, dvdy}.  n is set as given, not from dpdu x dpdv.
+        if (argc != 4) die("usage: differentials <req.bin> <out.bin>");
+        const std::vector<float> r = readFloats(argv[2]);
+        const size_t n = r.size() / 24;
+        std::vector<float> a(4 * n);
+        parallelRange(n, [&](size_t i) {
+            const float *c = &r[24 * i];
+            SurfaceInteraction si;
+            si.p = Point3f(c[0], c[1], c[2]);
+            si.n = Normal3f(c[3], c[4], c[5]);
+            si.dpdu = Vector3f(c[6], c[7], c[8]);
+            si.dpdv = Vector3f(c[9], c[10], c[11]);
+            RayDifferential ray(Point3f(0, 0, 0), Vector3f(0, 0, 1));
+            ray.hasDifferentials = true;
+            ray.rxOrigin = Point3f(c[12], c[13], c[14]);
+            ray.rxDirection = Vector3f(c[15], c[16], c[17]);
+            ray.ryOrigin = Point3f(c[18], c[19], c[20]);
+            ray.ryDirection = Vector3f(c[21], c[22], c[23]);
+            si.ComputeDifferentials(ray);
+            const float o[4] = {si.dudx, si.dvdx, si.dudy, si.dvdy};
+            memcpy(&a[4 * i], o, sizeof(o));
+        });
+        FILE *out = fopen(argv[3], "wb");
+        if (!out) die("cannot open output");
+        put(out, a.data(), 4 * a.size());
+        fclose(out);
+    } else if (cmd == "roughness") {
+        // roughness <lo> <hi>: RoughnessToAlpha of every float with bits in [lo, hi), written to stdout in chunks
+        if (argc != 4) die("usage: roughness <lo> <hi>");
+        const uint64_t lo = strtoull(argv[2], 0, 0), hi = strtoull(argv[3], 0, 0);
+        if (hi > (1ull << 32) || lo > hi) die("bad range");
+        std::vector<float> buf(1 << 20);
+        for (uint64_t s = lo; s < hi; s += buf.size()) {
+            const size_t m = (size_t)std::min<uint64_t>(buf.size(), hi - s);
+            for (size_t i = 0; i < m; ++i) {
+                const uint32_t b = (uint32_t)(s + i);
+                float x;
+                memcpy(&x, &b, 4);
+                buf[i] = TrowbridgeReitzDistribution::RoughnessToAlpha(x);
+            }
+            put(stdout, buf.data(), 4 * m);
+        }
+        fflush(stdout);
 #ifdef B200PT_PROBE_SPECTRAL
     } else if (cmd == "spectral") {
         // spectral <out.json-ish text>: everything liboracle_spectral needs from the SampledSpectrum build:

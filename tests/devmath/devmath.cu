@@ -2,6 +2,10 @@
 // for the product (same headers, same flags: csrc/nvflags.mk), and compares it bit for bit with the host's glibc (the
 // calls the reference makes) or with the host-compiled build of the same headers.  Loaded by tests/test_zz_devmath_gpu.py
 // (and, without a device, by tests/test_devmath.py for its host half) through ctypes.
+// Its texture half runs ImageTexture's MIPMap lookups, RoughnessToAlpha, InfiniteAreaLight's Le / Sample_Li / Pdf_Li
+// (pt_texture.cuh) and ComputeDifferentials (pt_core.cuh) on the device or host-compiled, over tables and queries the
+// reference's own classes answered (oracle/probe/ref_probe.cpp), for tests/test_zz_texlookup_gpu.py and
+// tests/test_texlookup.py.
 //
 // Pass rule: equal bits, or both outputs NaN (NaN payloads legitimately differ between the device and x86).
 // Device work goes in chunks of at most 256 MiB of outputs, and every call frees what it allocated.
@@ -15,6 +19,10 @@
 #include <vector>
 
 #include "pt_sphere.cuh"
+#if __has_include("pt_texture.cuh")
+#include "pt_texture.cuh"
+#define DM_TEXTURE 1
+#endif
 
 using namespace b200pt;
 
@@ -443,3 +451,322 @@ done:
 }
 
 }  // extern "C"
+
+#ifdef DM_TEXTURE
+// ---------------------------------------------------------------------------------------------------- textures and sky
+// One query per thread.  Query floats and answer words of each family:
+//   DM_T_EWA     {s, t, dst0.x, dst0.y, dst1.x, dst1.y} -> Lookup(st, dst0, dst1): r, g, b
+//   DM_T_WIDTH   {s, t, width}                          -> Lookup(st, width): r, g, b
+//   DM_T_SAMPLE  {u0, u1}                               -> Sample_Li: wi[3], pdf, Li[3], the visibility target[3]
+//   DM_T_PDF     {w[3]}                                 -> Pdf_Li
+//   DM_T_LE      {ray.d[3]}                             -> Le: r, g, b
+//   DM_T_DIFF    {p, n, dpdu, dpdv, rxOrigin, rxDirection, ryOrigin, ryDirection} -> dudx, dvdx, dudy, dvdy
+//   DM_T_ROUGH   {roughness}                            -> RoughnessToAlpha
+// A float MIPMap is uploaded as (v, v, v, 0) like b200pt_scene_add_mipmap does; its answers are compared on all three words.
+enum { DM_T_EWA = 0, DM_T_WIDTH, DM_T_SAMPLE, DM_T_PDF, DM_T_LE, DM_T_DIFF, DM_T_ROUGH, DM_T_N };
+static const int DM_T_IN[DM_T_N] = {6, 3, 2, 3, 3, 24, 1};
+static const int DM_T_OUT[DM_T_N] = {3, 3, 10, 1, 3, 4, 1};
+enum { DM_ON_HOST = 0, DM_ON_DEVICE = 1 };
+// The largest EWA bounding box (texels) a query may scan, and the largest |st * size| it may reach: beyond 2^31 the
+// device's (int)ceilf saturates where x86 gives INT_MIN, and a box ending at INT_MAX never ends (DESIGN.md, limits)
+#define DM_EWA_MAX_TEXELS 4096
+#define DM_ST_MAX 1073741824.f
+
+// The tables, as ref_probe returned them.  Levels: [h][w][channels] each, one after the other.
+extern "C" struct dm_mipmap {
+    int32_t channels, levels, wrap, trilinear;
+    float max_aniso;
+    int32_t w[B200PT_MIPMAP_MAX_LEVELS], h[B200PT_MIPMAP_MAX_LEVELS];
+    const float *texels;
+    float weight_lut[128];
+};
+extern "C" struct dm_sky {
+    int32_t w, h, nu, nv;
+    const float *texels;  // [h][w][3]
+    const float *cond_func, *cond_cdf, *cond_func_int, *marg_func, *marg_cdf;
+    float marg_func_int;
+    float light_to_world[16], world_to_light[16];
+    float two_world_radius;
+    float ref_p[3];
+};
+
+struct TexCtx {
+    DevMipmap M;
+    DevInfinite L;
+    float ref_p[3];
+};
+
+B200_HD void tex_eval(const TexCtx &c, int fam, const float *q, int nout, uint32_t *o) {
+    float f[10] = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+    switch (fam) {
+    case DM_T_EWA:
+    case DM_T_WIDTH: {
+        const Spec v = fam == DM_T_EWA ? mip_lookup(c.M, q[0], q[1], q[2], q[3], q[4], q[5]) : mip_lookup_width(c.M, q[0], q[1], q[2]);
+        f[0] = v.c[0], f[1] = v.c[1], f[2] = v.c[2];
+        break;
+    }
+    case DM_T_SAMPLE: {
+        V3 wi, pt;
+        float pdf;
+        const Spec li = infinite_sample_li(c.L, mk(c.ref_p[0], c.ref_p[1], c.ref_p[2]), q, &wi, &pdf, &pt);
+        const float r[10] = {wi.x, wi.y, wi.z, pdf, li.c[0], li.c[1], li.c[2], pt.x, pt.y, pt.z};
+        for (int k = 0; k < 10; ++k) f[k] = r[k];
+        break;
+    }
+    case DM_T_PDF: f[0] = infinite_pdf_li(c.L, mk(q[0], q[1], q[2])); break;
+    case DM_T_LE: {
+        const Spec v = infinite_le(c.L, mk(q[0], q[1], q[2]));
+        f[0] = v.c[0], f[1] = v.c[1], f[2] = v.c[2];
+        break;
+    }
+    case DM_T_DIFF: {
+        Isect is;
+        memset(&is, 0, sizeof(is));
+        is.p = mk(q[0], q[1], q[2]);
+        is.n = mk(q[3], q[4], q[5]);
+        TexGeom g;
+        memset(&g, 0, sizeof(g));
+        g.dpdu = mk(q[6], q[7], q[8]);
+        g.dpdv = mk(q[9], q[10], q[11]);
+        const V3 r[4] = {mk(q[12], q[13], q[14]), mk(q[15], q[16], q[17]), mk(q[18], q[19], q[20]), mk(q[21], q[22], q[23])};
+        compute_differentials(is, true, r, &g);
+        f[0] = g.dudx, f[1] = g.dvdx, f[2] = g.dudy, f[3] = g.dvdy;
+        break;
+    }
+    case DM_T_ROUGH: f[0] = roughness_to_alpha(q[0]); break;
+    }
+    for (int k = 0; k < nout; ++k) o[k] = float_as_uint(f[k]);
+}
+
+__global__ void k_tex(TexCtx c, int fam, int in, int out, const float *q, uint64_t n, uint32_t *o) {
+    const uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    tex_eval(c, fam, q + i * in, out, o + i * out);
+}
+
+// MIPMap::EWA's bounding box at `level` (the same arithmetic as mip_ewa), in texels; 0 past the last level
+static uint64_t ewa_box(const DevMipmap &M, int level, float st0, float st1, float d00, float d01, float d10, float d11) {
+    if (level >= M.levels) return 0;
+    const float w = (float)M.w[level], h = (float)M.h[level];
+    st0 = st0 * w - 0.5f;
+    st1 = st1 * h - 0.5f;
+    d00 *= w;
+    d01 *= h;
+    d10 *= w;
+    d11 *= h;
+    float A = d01 * d01 + d11 * d11 + 1;
+    float B = -2 * (d00 * d01 + d10 * d11);
+    float C = d00 * d00 + d10 * d10 + 1;
+    const float invF = 1 / (A * C - B * B * 0.25f);
+    A *= invF;
+    B *= invF;
+    C *= invF;
+    const float det = -B * B + 4 * A * C;
+    const float invDet = 1 / det;
+    const float uSqrt = sqrtf(det * C), vSqrt = sqrtf(A * det);
+    const float e[4] = {ceilf(st0 - 2 * invDet * uSqrt), floorf(st0 + 2 * invDet * uSqrt), ceilf(st1 - 2 * invDet * vSqrt),
+                        floorf(st1 + 2 * invDet * vSqrt)};
+    for (float v : e)
+        if (!(std::fabs(v) < DM_ST_MAX)) return UINT64_MAX;  // NaN included
+    const double ns = e[1] - e[0] + 1, nt = e[3] - e[2] + 1;
+    return ns > 0 && nt > 0 ? (uint64_t)(ns * nt) : 0;
+}
+// The texels mip_lookup scans for one EWA query: the boxes of the two levels its lod selects (MIPMap::Lookup's ellipse
+// clamp and lod, mipmap.h:276-303); UINT64_MAX when st or the box leaves the range the harness accepts
+static uint64_t ewa_footprint(const DevMipmap &M, const float *q) {
+    const int top = M.levels - 1;
+    if (!(std::fabs(q[0] * M.w[0]) < DM_ST_MAX && std::fabs(q[1] * M.h[0]) < DM_ST_MAX)) return UINT64_MAX;
+    if (M.trilinear) return 4;
+    float d00 = q[2], d01 = q[3], d10 = q[4], d11 = q[5];
+    if (d00 * d00 + d01 * d01 < d10 * d10 + d11 * d11) {
+        std::swap(d00, d10);
+        std::swap(d01, d11);
+    }
+    const float majorLength = sqrtf(d00 * d00 + d01 * d01);
+    float minorLength = sqrtf(d10 * d10 + d11 * d11);
+    if (minorLength * M.max_aniso < majorLength && minorLength > 0) {
+        const float scale = majorLength / (minorLength * M.max_aniso);
+        d10 *= scale;
+        d11 *= scale;
+        minorLength *= scale;
+    }
+    if (minorLength == 0) return 4;
+    const float lod = pt_max((float)0, top + pt_log2f(minorLength));
+    if (!(lod < 1e9f)) return UINT64_MAX;
+    const int ilod = (int)floorf(lod);
+    const uint64_t a = ewa_box(M, ilod, q[0], q[1], d00, d01, d10, d11), b = ewa_box(M, ilod + 1, q[0], q[1], d00, d01, d10, d11);
+    return a == UINT64_MAX || b == UINT64_MAX ? UINT64_MAX : std::max(a, b);
+}
+
+static DevMipmap host_mipmap(const dm_mipmap *m, std::vector<float4> *store) {
+    DevMipmap M;
+    memset(&M, 0, sizeof(M));
+    M.levels = m->levels;
+    M.wrap = m->wrap;
+    M.trilinear = m->trilinear;
+    M.max_aniso = m->max_aniso;
+    memcpy(M.weight_lut, m->weight_lut, sizeof(M.weight_lut));
+    size_t total = 0;
+    for (int l = 0; l < m->levels; ++l) total += (size_t)m->w[l] * m->h[l];
+    store->resize(total);
+    const float *src = m->texels;
+    size_t at = 0;
+    for (int l = 0; l < m->levels; ++l) {
+        M.w[l] = m->w[l];
+        M.h[l] = m->h[l];
+        M.texels[l] = store->data() + at;
+        for (size_t i = 0; i < (size_t)m->w[l] * m->h[l]; ++i, src += m->channels)
+            (*store)[at++] = m->channels == 3 ? make_float4(src[0], src[1], src[2], 0.f) : make_float4(src[0], src[0], src[0], 0.f);
+    }
+    return M;
+}
+
+static DevInfinite host_sky(const dm_sky *s, std::vector<float4> *store) {
+    DevInfinite L;
+    memset(&L, 0, sizeof(L));
+    L.w = s->w;
+    L.h = s->h;
+    store->resize((size_t)s->w * s->h);
+    for (size_t i = 0; i < store->size(); ++i)
+        (*store)[i] = make_float4(s->texels[3 * i], s->texels[3 * i + 1], s->texels[3 * i + 2], 0.f);
+    L.texels = store->data();
+    memcpy(L.light_to_world, s->light_to_world, sizeof(L.light_to_world));
+    memcpy(L.world_to_light, s->world_to_light, sizeof(L.world_to_light));
+    L.nu = s->nu;
+    L.nv = s->nv;
+    L.cond_func = s->cond_func;
+    L.cond_cdf = s->cond_cdf;
+    L.cond_func_int = s->cond_func_int;
+    L.marg_func = s->marg_func;
+    L.marg_cdf = s->marg_cdf;
+    L.marg_func_int = s->marg_func_int;
+    L.two_world_radius = s->two_world_radius;
+    return L;
+}
+
+// Copies n elements of src to a new device allocation recorded in `owned`
+template <class T>
+static cudaError_t upload(const T *src, size_t n, std::vector<void *> *owned, const T **dst) {
+    void *d = nullptr;
+    cudaError_t e = cudaMalloc(&d, std::max<size_t>(1, n) * sizeof(T));
+    if (e != cudaSuccess) return e;
+    owned->push_back(d);
+    *dst = (const T *)d;
+    return cudaMemcpy(d, src, n * sizeof(T), cudaMemcpyHostToDevice);
+}
+
+static int tex_run(int fam, const TexCtx &host, int where, const float *q, uint64_t n, const uint32_t *want, dm_report *rep,
+                   uint32_t *got, std::vector<void *> *owned, const std::vector<float4> &mipStore, const std::vector<float4> &skyStore,
+                   const dm_sky *sky) {
+    const int in = DM_T_IN[fam], out = DM_T_OUT[fam];
+    int rc = 0;
+    TexCtx dev = host;
+    float *dq = nullptr;
+    uint32_t *dout = nullptr;
+    std::vector<uint32_t> buf;
+    const uint64_t chunk = std::max<uint64_t>(1, std::min<uint64_t>(CHUNK_BYTES / (4 * (in + out)), n));
+    if (where == DM_ON_DEVICE) {
+        // the device copy of the tables: the same values, device pointers
+        if (host.M.levels > 0) {
+            const float4 *base = nullptr;
+            DM_CUDA(upload(mipStore.data(), mipStore.size(), owned, &base));
+            for (int l = 0; l < host.M.levels; ++l) dev.M.texels[l] = base + (host.M.texels[l] - mipStore.data());
+        }
+        if (sky) {
+            DM_CUDA(upload(skyStore.data(), skyStore.size(), owned, &dev.L.texels));
+            const size_t nu = sky->nu, nv = sky->nv;
+            DM_CUDA(upload(sky->cond_func, nu * nv, owned, &dev.L.cond_func));
+            DM_CUDA(upload(sky->cond_cdf, (nu + 1) * nv, owned, &dev.L.cond_cdf));
+            DM_CUDA(upload(sky->cond_func_int, nv, owned, &dev.L.cond_func_int));
+            DM_CUDA(upload(sky->marg_func, nv, owned, &dev.L.marg_func));
+            DM_CUDA(upload(sky->marg_cdf, nv + 1, owned, &dev.L.marg_cdf));
+        }
+        DM_CUDA(cudaMalloc(&dq, chunk * in * 4));
+        DM_CUDA(cudaMalloc(&dout, chunk * out * 4));
+    }
+    buf.resize(chunk * out);
+    for (uint64_t s = 0; s < n; s += chunk) {
+        const uint64_t m = std::min(chunk, n - s);
+        if (where == DM_ON_DEVICE) {
+            DM_CUDA(cudaMemcpy(dq, q + s * in, m * in * 4, cudaMemcpyHostToDevice));
+            k_tex<<<(unsigned)((m + 127) / 128), 128>>>(dev, fam, in, out, dq, m, dout);
+            DM_CUDA(cudaGetLastError());
+            DM_CUDA(cudaMemcpy(buf.data(), dout, m * out * 4, cudaMemcpyDeviceToHost));
+        } else {
+            uint32_t *b = buf.data();
+            parallel_for(m, [=, &host](uint64_t lo, uint64_t hi) {
+                for (uint64_t i = lo; i < hi; ++i) tex_eval(host, fam, q + (s + i) * in, out, b + i * out);
+            });
+        }
+        dm_compare(buf.data(), want + s * out, m * out, 0, s * out, 1, rep);
+        if (got) std::copy(buf.begin(), buf.begin() + m * out, got + s * out);
+    }
+done:
+    if (dq) cudaFree(dq);
+    if (dout) cudaFree(dout);
+    return rc;
+}
+
+static int free_all(std::vector<void *> &owned, int rc) {
+    for (void *p : owned) cudaFree(p);
+    return rc;
+}
+
+extern "C" {
+
+// Per EWA query (DM_T_EWA layout), the texels mip_lookup scans (the larger of its two levels' boxes); UINT64_MAX past the
+// accepted |st * size| range.  Host only: tests choose their queries with it.
+int dm_mip_footprint(const dm_mipmap *m, const float *q, uint64_t n, uint64_t *texels) {
+    std::vector<float4> store;
+    const DevMipmap M = host_mipmap(m, &store);
+    parallel_for(n, [&](uint64_t lo, uint64_t hi) {
+        for (uint64_t i = lo; i < hi; ++i) texels[i] = ewa_footprint(M, q + 6 * i);
+    });
+    return 0;
+}
+
+// MIPMap lookups (fam DM_T_EWA or DM_T_WIDTH) of n queries against want (3 words each), on the device or host-compiled.
+// The report's input is (query << 2) | word; got (optional) receives the words computed.  Refuses (-2) queries whose
+// EWA footprint exceeds DM_EWA_MAX_TEXELS or whose |st * size| reaches DM_ST_MAX, before anything runs.
+int dm_check_mip(const dm_mipmap *m, int fam, const float *q, uint64_t n, const uint32_t *want, int where, dm_report *rep,
+                 uint32_t *got) {
+    if ((fam != DM_T_EWA && fam != DM_T_WIDTH) || m->levels < 1 || m->levels > B200PT_MIPMAP_MAX_LEVELS) return -1;
+    TexCtx c;
+    memset(&c, 0, sizeof(c));
+    std::vector<float4> store;
+    c.M = host_mipmap(m, &store);
+    for (uint64_t i = 0; i < n; ++i) {
+        const float *e = q + (uint64_t)DM_T_IN[fam] * i;
+        if (!(std::fabs(e[0] * m->w[0]) < DM_ST_MAX && std::fabs(e[1] * m->h[0]) < DM_ST_MAX)) return -2;
+        if (fam == DM_T_EWA && ewa_footprint(c.M, e) > DM_EWA_MAX_TEXELS) return -2;
+    }
+    std::vector<void *> owned;
+    return free_all(owned, tex_run(fam, c, where, q, n, want, rep, got, &owned, store, {}, nullptr));
+}
+
+// InfiniteAreaLight queries (fam DM_T_SAMPLE, DM_T_PDF or DM_T_LE) against want, on the device or host-compiled; the
+// report's input is query * words + word.
+int dm_check_sky(const dm_sky *s, int fam, const float *q, uint64_t n, const uint32_t *want, int where, dm_report *rep,
+                 uint32_t *got) {
+    if ((fam != DM_T_SAMPLE && fam != DM_T_PDF && fam != DM_T_LE) || s->w < 1 || s->h < 1 || s->nu < 1 || s->nv < 1) return -1;
+    TexCtx c;
+    memset(&c, 0, sizeof(c));
+    std::vector<float4> store;
+    c.L = host_sky(s, &store);
+    memcpy(c.ref_p, s->ref_p, sizeof(c.ref_p));
+    std::vector<void *> owned;
+    return free_all(owned, tex_run(fam, c, where, q, n, want, rep, got, &owned, {}, store, s));
+}
+
+// ComputeDifferentials (DM_T_DIFF) or RoughnessToAlpha (DM_T_ROUGH) of n queries against want, on the device or
+// host-compiled; the report's input is query * words + word.
+int dm_check_geom(int fam, const float *q, uint64_t n, const uint32_t *want, int where, dm_report *rep, uint32_t *got) {
+    if (fam != DM_T_DIFF && fam != DM_T_ROUGH) return -1;
+    TexCtx c;
+    memset(&c, 0, sizeof(c));
+    std::vector<void *> owned;
+    return free_all(owned, tex_run(fam, c, where, q, n, want, rep, got, &owned, {}, {}, nullptr));
+}
+
+}  // extern "C"
+#endif  // DM_TEXTURE
