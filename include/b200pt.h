@@ -163,8 +163,8 @@ typedef struct b200pt_instance {
  * values (shapes/triangle.cpp:73-75) gathered through the index buffer:
  * 9 floats per triangle (p0 p1 p2).  Per-vertex shading normals (TriangleMesh::n,
  * world space) and uvs (TriangleMesh::uv) are optional, gathered the same way;
- * per-vertex tangents (s) and alpha masks are out of scope and must be rejected
- * by the host. */
+ * per-vertex tangents (s) are out of scope and must be rejected by the host.
+ * Alpha masks are set after creation (b200pt_scene_set_alpha_masks). */
 typedef struct b200pt_scene_desc {
     int64_t n_triangles;
     const float *vertices;        /* [n_triangles][3][3]                              */
@@ -413,6 +413,27 @@ int b200pt_scene_add_mipmap(b200pt_scene *scene, const b200pt_mipmap *desc, int3
  * the material's "remaproughness" (roughness slots only: the looked-up value goes through RoughnessToAlpha). */
 int b200pt_scene_bind_texture(b200pt_scene *scene, int32_t material, int32_t slot, int32_t mipmap, float su, float sv,
                               float du, float dv, int32_t remap_roughness);
+
+/* ---- alpha masks: TriangleMesh::alphaMask / shadowAlphaMask (shapes/triangle.cpp:718-743), evaluated inside
+ * Triangle::Intersect and IntersectP.  There the texture is looked up without differentials, which for an ImageTexture
+ * under UVMapping2D is the bilinear lookup of pyramid level 0 (MIPMap::triangle(0, st)): level 0 is all the device needs.
+ * A candidate hit is rejected when a mask is exactly 0 there: closest hits test alpha; any-hit rays (b200pt_trace_any,
+ * the path integrator's shadow rays) test alpha and shadowalpha; the volpath integrator's shadow rays test alpha only,
+ * as its Tr() intersects with Intersect.  Shape::Pdf and Shape::Sample ignore masks, and so does the device.  Works on
+ * RGBSpectrum and SampledSpectrum scenes alike. */
+typedef struct b200pt_alpha_mask {
+    int32_t width, height;          /* mipmap->pyramid[0]: uSize(), vSize(); 0 x 0 with texels NULL: ConstantTexture(0) */
+    const float *texels;            /* [height][width] one float channel                                                 */
+    int32_t wrap;                   /* B200PT_WRAP_*                                                                     */
+    float su, sv, du, dv;           /* UVMapping2D                                                                       */
+} b200pt_alpha_mask;
+/* Copies the mask to the device; *id names it in b200pt_scene_set_alpha_masks.  The device keeps each texel as a float4
+ * (the layout of the image-texture lookups it shares), 16 bytes per texel: 64 MB for a 2048 x 2048 mask. */
+int b200pt_scene_add_alpha_mask(b200pt_scene *scene, const b200pt_alpha_mask *desc, int32_t *id);
+/* Per triangle of the scene's numbering (b200pt_scene_desc, n_triangles entries each): the alpha and the shadowalpha
+ * mask, or -1; either array may be NULL (no mask of that kind).  A later call replaces the earlier one.  Both entry
+ * points must be called before the scene's first trace or b200pt_render_create. */
+int b200pt_scene_set_alpha_masks(b200pt_scene *scene, const int32_t *alpha, const int32_t *shadow_alpha);
 
 /* ---- kernel-level entry points (parity tests, traversal benchmarks) -------
  * Replace Scene::Intersect / Scene::IntersectP (core/scene.cpp:45-55) on

@@ -44,6 +44,8 @@ _SIGNATURES = {
     "b200pt_scene_set_infinite_light": (C.c_int, [_vp, _i32, C.POINTER(abi.InfiniteLight)]),
     "b200pt_scene_add_mipmap": (C.c_int, [_vp, C.POINTER(abi.Mipmap), C.POINTER(_i32)]),
     "b200pt_scene_bind_texture": (C.c_int, [_vp, _i32, _i32, _i32, C.c_float, C.c_float, C.c_float, C.c_float, _i32]),
+    "b200pt_scene_add_alpha_mask": (C.c_int, [_vp, C.POINTER(abi.AlphaMask), C.POINTER(_i32)]),
+    "b200pt_scene_set_alpha_masks": (C.c_int, [_vp, _vp, _vp]),
     "b200pt_trace_closest": (C.c_int, [_vp, _vp, _vp, _i64]),
     "b200pt_trace_any": (C.c_int, [_vp, _vp, _vp, _i64]),
     "b200pt_trace_closest_dev": (C.c_int, [_vp, _u64, _u64, _i64]),
@@ -162,6 +164,7 @@ class Scene:
         self.ctx = ctx
         self._keep = keepalive
         self.h = _vp()
+        self.n_triangles = int(desc.n_triangles)
         _check(lib.b200pt_scene_create(ctx.h, C.byref(desc), C.byref(self.h)))
 
     def upload(self):
@@ -211,6 +214,34 @@ class Scene:
         of material `material`."""
         _check(lib.b200pt_scene_bind_texture(self.h, int(material), int(slot), int(mipmap), su, sv, du, dv,
                                              1 if remap_roughness else 0))
+
+    def add_alpha_mask(self, texels=None, wrap=abi.WRAP_REPEAT, su=1.0, sv=1.0, du=0.0, dv=0.0):
+        """b200pt_scene_add_alpha_mask: `texels` is level 0 of the mask's MIPMap, [h][w]; None is ConstantTexture(0).
+        Returns the mask's id.  The library copies the texels."""
+        rec = abi.AlphaMask()
+        arr = None
+        if texels is not None:
+            arr = np.ascontiguousarray(texels, dtype=np.float32)
+            if arr.ndim != 2:
+                raise ValueError("an alpha mask is one float channel, [h][w]")
+            rec.height, rec.width = arr.shape
+            rec.texels = arr.ctypes.data
+        rec.wrap, rec.su, rec.sv, rec.du, rec.dv = int(wrap), su, sv, du, dv
+        out = _i32()
+        _check(lib.b200pt_scene_add_alpha_mask(self.h, C.byref(rec), C.byref(out)))
+        return out.value
+
+    def set_alpha_masks(self, alpha=None, shadow_alpha=None):
+        """b200pt_scene_set_alpha_masks: per triangle of the scene's numbering, the alpha / shadowalpha mask id or -1
+        (None: no mask of that kind).  Before the scene's first trace or render."""
+        arrs = []
+        for a in (alpha, shadow_alpha):
+            if a is not None:
+                a = np.ascontiguousarray(a, dtype=np.int32)
+                if a.shape != (self.n_triangles,):
+                    raise ValueError("set_alpha_masks: %s ids for %d triangles" % (a.shape, self.n_triangles))
+            arrs.append(a)
+        _check(lib.b200pt_scene_set_alpha_masks(self.h, abi.ptr(arrs[0]), abi.ptr(arrs[1])))
 
     def trace_closest(self, rays):
         rays = np.ascontiguousarray(rays, dtype=abi.RAY_DTYPE)

@@ -87,6 +87,12 @@ class Mipmap(C.Structure):
                 ("trilinear", C.c_int32), ("max_anisotropy", C.c_float), ("weight_lut", C.c_float * 128)]
 
 
+class AlphaMask(C.Structure):
+    """b200pt_alpha_mask: level 0 of an alpha / shadowalpha mask's MIPMap under UVMapping2D (0 x 0, no texels: constant 0)."""
+    _fields_ = [("width", C.c_int32), ("height", C.c_int32), ("texels", C.c_void_p), ("wrap", C.c_int32),
+                ("su", C.c_float), ("sv", C.c_float), ("du", C.c_float), ("dv", C.c_float)]
+
+
 class SamplerDesc(C.Structure):
     _fields_ = [("samples_per_pixel", C.c_int32), ("sample_bounds", C.c_int32 * 4),
                 ("n_dimensions", C.c_int32), ("matrices32", C.c_void_p), ("vdc", C.c_void_p),

@@ -96,6 +96,13 @@ struct b200pt_scene {
     std::vector<int> mipmap_channels;
     std::vector<void *> d_mipmap_texels;
     std::vector<DevTexBind> tex_bind;
+    // alpha masks (b200pt_scene_add_alpha_mask / b200pt_scene_set_alpha_masks): d_alpha_masks is nullptr until masks are
+    // set on some triangle; `used` is set by the first trace or render_create, after which the masks are fixed
+    std::vector<DevAlphaMask> alpha_masks;
+    std::vector<void *> d_alpha_texels;
+    DevAlphaMask *d_alpha_masks = nullptr;
+    int32_t *d_alpha_ids = nullptr;
+    bool used = false;
 };
 
 struct TimedLaunch {
@@ -168,6 +175,10 @@ static void trace_args_scene(TraceArgs &a, const b200pt_scene *s) {
     a.bounds = s->trav_bounds;
     a.tlas_bounds = s->tlas_bounds;
     a.tris = s->d_tris;
+    a.alpha_masks = s->d_alpha_masks;
+    a.alpha_ids = s->d_alpha_ids;
+    a.tri_uv = s->d_tri_uv;
+    a.alpha_any_shadow = 1;
 }
 // the members every traversal launch of a render shares: the tree's, plus the per-slot record stride and the k_trace knobs;
 // everything else zero
@@ -180,6 +191,7 @@ static TraceArgs trace_args_render(const b200pt_render *r) {
     a.stride = REC_F4;
     a.refill_lanes = r->refill_lanes;
     a.postpone_pct = r->postpone_pct;
+    a.alpha_any_shadow = r->host.volpath ? 0 : 1;  // VolPathIntegrator's shadow rays go through Tr (Intersect), path's through Unoccluded
     return a;
 }
 
@@ -711,6 +723,9 @@ void b200pt_scene_destroy(b200pt_scene *s) {
     cudaFree(s->d_work);
     for (void *p : s->d_infinite_tables) cudaFree(p);
     for (void *p : s->d_mipmap_texels) cudaFree(p);
+    for (void *p : s->d_alpha_texels) cudaFree(p);
+    cudaFree(s->d_alpha_masks);
+    cudaFree(s->d_alpha_ids);
     cudaFreeHost(s->h_nodes);
     cudaFreeHost(s->h_tri_base);
     cudaFreeHost(s->h_tris);
@@ -877,6 +892,89 @@ int b200pt_scene_bind_texture(b200pt_scene *s, int32_t material, int32_t slot, i
     return B200PT_OK;
 }
 
+int b200pt_scene_add_alpha_mask(b200pt_scene *s, const b200pt_alpha_mask *d, int32_t *id) {
+    if (!s || !d || !id) return b200pt_fail(B200PT_ERR_INVALID, "scene_add_alpha_mask: NULL argument");
+    if (s->used) return b200pt_fail(B200PT_ERR_INVALID, "scene_add_alpha_mask: the scene was already traced or rendered");
+    const bool constant = d->width == 0 && d->height == 0 && !d->texels;
+    if (!constant) {
+        if (d->width <= 0 || d->height <= 0 || (int64_t)d->width * d->height > (1ll << 28))
+            return b200pt_fail(B200PT_ERR_INVALID, "scene_add_alpha_mask: bad size %d x %d", d->width, d->height);
+        if (!d->texels) return b200pt_fail(B200PT_ERR_INVALID, "scene_add_alpha_mask: texels are NULL");
+        if (d->wrap < B200PT_WRAP_REPEAT || d->wrap > B200PT_WRAP_CLAMP)
+            return b200pt_fail(B200PT_ERR_INVALID, "scene_add_alpha_mask: unknown wrap mode %d", d->wrap);
+    }
+    DevAlphaMask M;
+    memset(&M, 0, sizeof(M));
+    M.su = d->su;
+    M.sv = d->sv;
+    M.du = d->du;
+    M.dv = d->dv;
+    float4 *dp = nullptr;
+    if (!constant) {
+        CUDA_TRY(cudaSetDevice(s->ctx->device));
+        const size_t n = (size_t)d->width * d->height;
+        std::vector<float4> h(n);
+        for (size_t i = 0; i < n; ++i) h[i] = make_float4(d->texels[i], d->texels[i], d->texels[i], 0.f);
+        if (cudaMalloc(&dp, n * sizeof(float4)) != cudaSuccess)
+            return b200pt_fail(B200PT_ERR_OOM, "scene_add_alpha_mask: cudaMalloc of %zu bytes failed", n * sizeof(float4));
+        if (cudaMemcpy(dp, h.data(), n * sizeof(float4), cudaMemcpyHostToDevice) != cudaSuccess) {
+            cudaFree(dp);
+            return b200pt_fail(B200PT_ERR_CUDA, "scene_add_alpha_mask: upload failed");
+        }
+        M.mip.levels = 1;
+        M.mip.wrap = d->wrap;
+        M.mip.w[0] = d->width;
+        M.mip.h[0] = d->height;
+        M.mip.texels[0] = dp;
+    }
+    *id = (int32_t)s->alpha_masks.size();
+    s->alpha_masks.push_back(M);
+    s->d_alpha_texels.push_back(dp);
+    return B200PT_OK;
+}
+
+int b200pt_scene_set_alpha_masks(b200pt_scene *s, const int32_t *alpha, const int32_t *shadow_alpha) {
+    if (!s) return b200pt_fail(B200PT_ERR_INVALID, "scene_set_alpha_masks: scene is NULL");
+    if (s->used) return b200pt_fail(B200PT_ERR_INVALID, "scene_set_alpha_masks: the scene was already traced or rendered");
+    const int64_t n = (int64_t)s->n_prims, nm = (int64_t)s->alpha_masks.size();
+    std::vector<int32_t> ids((size_t)n * 2, -1);
+    bool any = false;
+    for (int64_t i = 0; i < n; ++i)
+        for (int k = 0; k < 2; ++k) {
+            const int32_t *arr = k ? shadow_alpha : alpha;
+            if (!arr) continue;
+            if (arr[i] < -1 || arr[i] >= nm)
+                return b200pt_fail(B200PT_ERR_INVALID, "scene_set_alpha_masks: %s mask %d of triangle %lld out of range (%lld masks)",
+                                   k ? "shadowalpha" : "alpha", arr[i], (long long)i, (long long)nm);
+            ids[(size_t)i * 2 + k] = arr[i];
+            any = any || arr[i] >= 0;
+        }
+    CUDA_TRY(cudaSetDevice(s->ctx->device));
+    // h_tris may still be the source of b200pt_scene_upload's asynchronous copy on the context's stream
+    CUDA_TRY(cudaStreamSynchronize(s->ctx->stream));
+    cudaFree(s->d_alpha_masks);
+    cudaFree(s->d_alpha_ids);
+    s->d_alpha_masks = nullptr;
+    s->d_alpha_ids = nullptr;
+    // the flag word of each triangle record (host SAH and device LBVH builds alike: h_tris holds either)
+    TriRecord *t = static_cast<TriRecord *>(s->h_tris);
+    for (uint64_t i = 0; i < s->n_tris; ++i) t[i].mat_flags &= ~B200PT_TRI_ALPHA;
+    if (any) {
+        for (int64_t i = 0; i < n; ++i)
+            if (ids[(size_t)i * 2] >= 0 || ids[(size_t)i * 2 + 1] >= 0) t[s->prim_to_tri[(size_t)i]].mat_flags |= B200PT_TRI_ALPHA;
+        if (cudaMalloc(&s->d_alpha_masks, nm * sizeof(DevAlphaMask)) != cudaSuccess ||
+            cudaMalloc(&s->d_alpha_ids, ids.size() * sizeof(int32_t)) != cudaSuccess) {
+            cudaFree(s->d_alpha_masks);
+            s->d_alpha_masks = nullptr;
+            return b200pt_fail(B200PT_ERR_OOM, "scene_set_alpha_masks: cudaMalloc failed");
+        }
+        CUDA_TRY(cudaMemcpy(s->d_alpha_masks, s->alpha_masks.data(), nm * sizeof(DevAlphaMask), cudaMemcpyHostToDevice));
+        CUDA_TRY(cudaMemcpy(s->d_alpha_ids, ids.data(), ids.size() * sizeof(int32_t), cudaMemcpyHostToDevice));
+    }
+    CUDA_TRY(cudaMemcpy(s->d_tris, s->h_tris, s->n_tris * sizeof(TriRecord), cudaMemcpyHostToDevice));
+    return B200PT_OK;
+}
+
 int b200pt_scene_info(const b200pt_scene *s, uint64_t *node_bytes, uint64_t *tri_bytes, uint64_t *n_nodes) {
     if (!s) return b200pt_fail(B200PT_ERR_INVALID, "scene is NULL");
     if (node_bytes) *node_bytes = s->n_nodes * (sizeof(WbvhNode) + sizeof(uint32_t));
@@ -916,6 +1014,7 @@ static bool two_level(const b200pt_scene *s) {
 static int trace_dev(b200pt_scene *s, uint64_t rays_dev, uint64_t out_dev, int64_t n, bool any_hit) {
     if (!s) return b200pt_fail(B200PT_ERR_INVALID, "scene is NULL");
     if (n < 0 || n >= (1ll << 32)) return b200pt_fail(B200PT_ERR_INVALID, "trace: bad ray count");
+    s->used = true;
     if (n == 0) return B200PT_OK;
     CUDA_TRY(cudaSetDevice(s->ctx->device));
     cudaStream_t st = s->ctx->stream;
@@ -1019,6 +1118,7 @@ extern "C" {
 int b200pt_render_create(b200pt_scene *scene, const b200pt_camera_desc *cam, const b200pt_film_desc *film,
                          const b200pt_sampler_desc *smp, const b200pt_integrator_desc *integ, b200pt_render **out) {
     if (!scene || !cam || !film || !smp || !integ || !out) return b200pt_fail(B200PT_ERR_INVALID, "render_create: NULL argument");
+    scene->used = true;
     if (!(film->filter_radius[0] > 0.f) || !(film->filter_radius[1] > 0.f) || film->filter_radius[0] > 8.f ||
         film->filter_radius[1] > 8.f)
         return b200pt_fail(B200PT_ERR_INVALID, "render_create: pixel filter radius must be in (0, 8]");

@@ -62,6 +62,14 @@ struct DevTexBind {
     int remap;             // roughness slots: RoughnessToAlpha after the lookup
 };
 
+// An alpha / shadowalpha mask (b200pt_alpha_mask): ImageTexture<Float, Float> under UVMapping2D, or ConstantTexture(0)
+// (mip.levels == 0).  Inside intersection the texture is evaluated without differentials, which is the bilinear lookup of
+// level 0 (MIPMap::triangle(0, st)), so only level 0 is kept, as a one-level DevMipmap.
+struct DevAlphaMask {
+    DevMipmap mip;
+    float su, sv, du, dv;  // UVMapping2D
+};
+
 struct DevScene {
     const U4 *nodes;
     const uint32_t *tri_base;  // per node: first triangle of its leaf children (wbvh.h)
@@ -269,6 +277,11 @@ struct TraceArgs {
     uint32_t n_instances;
     uint32_t tlas_node_off, tlas_tri_off;  // see DevScene
     uint32_t *hit_inst_out;     // instance of an object-triangle hit (closest, render path)
+    // alpha masks (b200pt_scene_set_alpha_masks); nullptr: the scene has none and the launchers run the unmasked kernels
+    const DevAlphaMask *alpha_masks;
+    const int32_t *alpha_ids;   // [n_triangles][2] in the scene's numbering (TriRecord::prim): alpha, shadowalpha mask or -1
+    const F4 *tri_uv;           // see DevScene
+    int alpha_any_shadow;       // any-hit rays also test shadowalpha (IntersectP); 0: alpha only (volpath's Tr)
 };
 // the entry of `slot` in a traversal output: a field of the per-slot records or an element of a plain array
 template <class T>

@@ -63,6 +63,7 @@ static_assert(sizeof(WbvhNode) == 64, "WbvhNode must be 64 bytes");
 #define B200PT_TRI_HAS_NORMALS 0x40000u  // per-vertex shading normals in DevScene::tri_n
 #define B200PT_TRI_HAS_UVS 0x80000u      // uvs in DevScene::tri_uv
 #define B200PT_TRI_INSTANCED 0x100000u   // object-space triangle of an instanced object
+#define B200PT_TRI_ALPHA 0x200000u       // the mesh has an alpha or shadowalpha mask (b200pt_scene_set_alpha_masks)
 
 struct alignas(16) TriRecord {  // 48 bytes
     float p0[3];

@@ -361,9 +361,19 @@ B200_HD void leaf_group_triangles(const uint32_t *__restrict__ tri_base, uint32_
     *tg_y = bits;
 }
 
-template <bool ANY_HIT, bool COUNT>
+// Triangles without alpha masks: the watertight test alone decides.  Every scene without masks runs this.
+struct NoAlpha {
+    static constexpr bool enabled = false;
+    B200_HD NoAlpha at(uint32_t) const { return *this; }
+    B200_HD bool rejects(bool, uint32_t, uint32_t, uint32_t, const TriHit &) const { return false; }
+};
+
+// ALPHA (see AlphaTest in kernels.cu) rejects a candidate the test accepted when its mesh's mask evaluates to exactly 0
+// (Triangle::Intersect / IntersectP, shapes/triangle.cpp:332-337, 531-570).  A rejected candidate does not shorten the ray.
+// Only triangles flagged B200PT_TRI_ALPHA are looked up, from the flag word the test loads anyway.
+template <bool ANY_HIT, bool COUNT, class ALPHA = NoAlpha>
 B200_HD bool trav_tri_phase(TravRay &R, const uint32_t *__restrict__ tri_base, const F4 *__restrict__ tris, uint32_t lg_x,
-                            uint32_t lg_y, TraceCounters *ctr) {
+                            uint32_t lg_y, TraceCounters *ctr, const ALPHA &alpha = ALPHA()) {
     uint32_t tg_x, tg_y;
     leaf_group_triangles(tri_base, lg_x, lg_y, &tg_x, &tg_y);
     while (tg_y) {
@@ -375,6 +385,9 @@ B200_HD bool trav_tri_phase(TravRay &R, const uint32_t *__restrict__ tri_base, c
         if (COUNT) ctr->tris++;
         TriHit h;
         if (triangle_test(mk(v0.x, v0.y, v0.z), mk(v1.x, v1.y, v1.z), mk(v2.x, v2.y, v2.z), R.o, R.sh, R.tmax, &h)) {
+            if (ALPHA::enabled && (float_as_uint(v1.w) & B200PT_TRI_ALPHA) &&
+                alpha.rejects(ANY_HIT, ti, float_as_uint(v0.w), float_as_uint(v1.w), h))
+                continue;
             R.tmax = h.t;  // primitive.cpp:120 (the caller rescales the box parameter: trav_rescale)
             R.best = ti;
             R.hit = h;
@@ -396,13 +409,13 @@ B200_HD bool trav_next_group(Trav &T, TravStack &S) {
 
 // One complete step (node phase, then its triangles at once).  Returns true when the traversal
 // is complete (closest hit known / any hit found / nothing left).
-template <bool ANY_HIT, bool COUNT>
+template <bool ANY_HIT, bool COUNT, class ALPHA = NoAlpha>
 B200_HD bool trav_step(Trav &T, TravRay &R, TravStack &S, const U4 *__restrict__ nodes, const uint32_t *__restrict__ tri_base,
-                        const F4 *__restrict__ tris, const uint8_t *lut, TraceCounters *ctr) {
+                        const F4 *__restrict__ tris, const uint8_t *lut, TraceCounters *ctr, const ALPHA &alpha = ALPHA()) {
     uint32_t tg_x = 0, tg_y = 0;
     if (T.cur_y & 0xff000000u) trav_node_phase<!ANY_HIT, COUNT>(T, S, nodes, tri_base, lut, &tg_x, &tg_y, ctr);
     const float before = R.tmax;
-    if (trav_tri_phase<ANY_HIT, COUNT>(R, tri_base, tris, tg_x, tg_y, ctr)) return true;
+    if (trav_tri_phase<ANY_HIT, COUNT>(R, tri_base, tris, tg_x, tg_y, ctr, alpha)) return true;
     if (R.tmax != before) trav_rescale(T, R, R.tmax);
     return !trav_next_group(T, S);
 }
@@ -410,16 +423,16 @@ B200_HD bool trav_step(Trav &T, TravRay &R, TravStack &S, const U4 *__restrict__
 // Whole traversal of one ray (used by the CPU pre-flight and the simple entry points).
 // Returns the leaf-order index of the closest (ANY_HIT: of some) hit triangle or
 // B200PT_MISS; *hit receives (t, b0, b1, b2) of the accepted intersection.
-template <bool ANY_HIT, bool COUNT>
+template <bool ANY_HIT, bool COUNT, class ALPHA = NoAlpha>
 B200_HD uint32_t traverse_wbvh(const U4 *__restrict__ nodes, const uint32_t *__restrict__ tri_base, const F4 *__restrict__ tris,
                                const TravBounds &B, const uint8_t *lut, const V3 &o, const V3 &d, float rayTMax, TriHit *hit,
-                               TraceCounters *ctr, uint32_t *overflow = nullptr) {
+                               TraceCounters *ctr, uint32_t *overflow = nullptr, const ALPHA &alpha = ALPHA()) {
     Trav T;
     TravRay R;
     TravStack S;
     trav_init(T, R, o, d, rayTMax, B);
     if (T.cur_y & 0xff000000u)
-        while (!trav_step<ANY_HIT, COUNT>(T, R, S, nodes, tri_base, tris, lut, ctr)) {
+        while (!trav_step<ANY_HIT, COUNT>(T, R, S, nodes, tri_base, tris, lut, ctr, alpha)) {
         }
     *hit = R.hit;
     if (overflow && (T.sp & B200PT_SP_OVERFLOW)) *overflow += 1;

@@ -184,6 +184,16 @@ struct Flattened {
         int remap;
     };
     std::vector<Bind> binds;
+    // alpha / shadowalpha masks (b200pt_scene_add_alpha_mask / b200pt_scene_set_alpha_masks): every distinct mask
+    // texture once (w == 0: ConstantTexture(0)), and per triangle its masks or -1
+    struct Alpha {
+        int w, h, wrap;
+        float su, sv, du, dv;
+        std::vector<float> texels;
+    };
+    std::vector<Alpha> alphaMasks;
+    std::unordered_map<const void *, int> alphaOf;
+    std::vector<int32_t> alphaId, shadowAlphaId;
 };
 
 // The MIPMap of an ImageTexture as the host built it (mipmap.h:116-218): the levels, the wrap mode, the filter settings
@@ -230,6 +240,48 @@ bool TexturedParam(const std::shared_ptr<Texture<T>> &tex, T *value, int materia
     f->binds.push_back({material, slot, AddMipmap(it->mipmap, f), uv->su, uv->sv, uv->du, uv->dv, remap});
     return true;
 }
+// A mesh's alphaMask or shadowAlphaMask (triangle.cpp:718-743): *id = -1 for none, else the mask.  Inside
+// Triangle::Intersect / IntersectP the texture is evaluated without differentials, so an ImageTexture<Float, Float> under
+// UVMapping2D reads level 0 of its MIPMap only (copied, nothing recomputed).  A constant that is not 0 never rejects a
+// hit; IntersectP's rejection of masked triangles with a zero geometric normal needs no mask either, since such
+// triangles never enter the device's trees.
+bool AlphaMask(const std::shared_ptr<Texture<Float>> &tex, Flattened *f, int32_t *id, std::string *why) {
+    *id = -1;
+    if (!tex) return true;
+    auto found = f->alphaOf.find(tex.get());
+    if (found != f->alphaOf.end()) return *id = found->second, true;
+    Flattened::Alpha a;
+    a.w = a.h = 0;
+    a.wrap = B200PT_WRAP_REPEAT;
+    a.su = a.sv = 1.f;
+    a.du = a.dv = 0.f;
+    Float c;
+    if (ConstantValue(tex, &c)) {
+        if (c != 0) return true;
+    } else {
+        auto it = dynamic_cast<const ImageTexture<Float, Float> *>(tex.get());
+        if (!it) return *why = "alpha masks other than \"constant\" and \"imagemap\" textures", false;
+        auto uv = dynamic_cast<const UVMapping2D *>(it->mapping.get());
+        if (!uv) return *why = "alpha masks with a mapping other than \"uv\"", false;
+        const MIPMap<Float> *mm = it->mipmap;
+        const auto &lv = *mm->pyramid[0];
+        a.w = lv.uSize();
+        a.h = lv.vSize();
+        a.wrap = mm->wrapMode == ImageWrap::Repeat ? B200PT_WRAP_REPEAT : mm->wrapMode == ImageWrap::Black ? B200PT_WRAP_BLACK : B200PT_WRAP_CLAMP;
+        a.su = uv->su;
+        a.sv = uv->sv;
+        a.du = uv->du;
+        a.dv = uv->dv;
+        a.texels.reserve((size_t)a.w * a.h);
+        for (int y = 0; y < a.h; ++y)
+            for (int x = 0; x < a.w; ++x) a.texels.push_back(lv(x, y));
+    }
+    *id = (int32_t)f->alphaMasks.size();
+    f->alphaMasks.push_back(std::move(a));
+    f->alphaOf[tex.get()] = *id;
+    return true;
+}
+
 bool SpectrumParam(const std::shared_ptr<Texture<Spectrum>> &tex, Spectrum *value, int material, int slot, Flattened *f, std::string *why) {
     return TexturedParam<Spectrum, RGBSpectrum>(tex, value, material, slot, 0, f, why);
 }
@@ -363,8 +415,11 @@ bool FlattenScene(const Scene &scene, Flattened *f, std::string *why, bool volum
         if (!volumetric && (gp->mediumInterface.inside || gp->mediumInterface.outside)) return *why = "participating media", false;
         if (!noTransition(gp)) return false;
         const TriangleMesh &mesh = *tri->mesh;
-        if (mesh.s || mesh.alphaMask || mesh.shadowAlphaMask)
-            return *why = "meshes with per-vertex tangents / alpha masks", false;
+        if (mesh.s) return *why = "meshes with per-vertex tangents", false;
+        int32_t alpha, shadowAlpha;
+        if (!AlphaMask(mesh.alphaMask, f, &alpha, why) || !AlphaMask(mesh.shadowAlphaMask, f, &shadowAlpha, why)) return false;
+        f->alphaId.push_back(alpha);
+        f->shadowAlphaId.push_back(shadowAlpha);
         for (int v = 0; v < 3; ++v) {
             const Point3f &p = mesh.p[tri->v[v]];
             f->vertices.push_back(p.x);
@@ -840,6 +895,21 @@ class GpuIntegrator : public Base {
                         fwrite(&b.remap, 4, 1, df);
                     }
                 }
+                // alpha masks (appended after the texture tables, behind their own marker): the masks, then per triangle
+                // the alpha and the shadowalpha mask ids
+                if (!flat.alphaMasks.empty()) {
+                    const int32_t ah[2] = {-3, (int32_t)flat.alphaMasks.size()};
+                    fwrite(ah, 4, 2, df);
+                    for (const auto &a : flat.alphaMasks) {
+                        const int32_t mh[3] = {a.w, a.h, a.wrap};
+                        const float mf[4] = {a.su, a.sv, a.du, a.dv};
+                        fwrite(mh, 4, 3, df);
+                        fwrite(mf, 4, 4, df);
+                        fwrite(a.texels.data(), 4, a.texels.size(), df);
+                    }
+                    fwrite(flat.alphaId.data(), 4, flat.alphaId.size(), df);
+                    fwrite(flat.shadowAlphaId.data(), 4, flat.shadowAlphaId.size(), df);
+                }
                 fclose(df);
             }
         }
@@ -906,6 +976,23 @@ class GpuIntegrator : public Base {
         }
         for (const auto &b : flat.binds)
             B200_CHECK(b200pt_scene_bind_texture(gscene, b.material, b.slot, mipIds[b.mip], b.su, b.sv, b.du, b.dv, b.remap));
+        if (!flat.alphaMasks.empty()) {
+            for (const auto &a : flat.alphaMasks) {
+                b200pt_alpha_mask am;
+                memset(&am, 0, sizeof(am));
+                am.width = a.w;
+                am.height = a.h;
+                am.texels = a.w ? a.texels.data() : nullptr;
+                am.wrap = a.wrap;
+                am.su = a.su;
+                am.sv = a.sv;
+                am.du = a.du;
+                am.dv = a.dv;
+                int32_t aid = -1;
+                B200_CHECK(b200pt_scene_add_alpha_mask(gscene, &am, &aid));  // ids follow the order of the calls
+            }
+            B200_CHECK(b200pt_scene_set_alpha_masks(gscene, flat.alphaId.data(), flat.shadowAlphaId.data()));
+        }
         B200_CHECK(b200pt_render_create(gscene, &cd, &fd, &smpd, &id, &render));
         B200_CHECK(b200pt_ctx_synchronize(ctx));
         const auto t2 = now();

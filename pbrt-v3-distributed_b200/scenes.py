@@ -140,7 +140,7 @@ class SceneArrays:
 
     def __init__(self, n_tris, materials=("matte",), soup_version=1, seed=1234, light_L=40.0,
                  n_lights=None, two_sided=False, reverse_orientation=(), shading_normals=(), uvs=(), spheres=(),
-                 objects=(), instances=(), delta_lights=(), infinite_lights=(), textures=None):
+                 objects=(), instances=(), delta_lights=(), infinite_lights=(), textures=None, alphas=None):
         """spheres: dicts {center, radius, material (a name in `materials` or "black"), emit (radiance or
         None), scale (sx, sy, sz) or None, reverse_orientation} -- written as `Translate` + `Scale` +
         `Shape "sphere"` by write_pbrt, after the meshes."""
@@ -227,6 +227,11 @@ class SceneArrays:
         # gamma, uscale, vscale, udelta, vdelta}; write_pbrt declares them as imagemap textures under the "uv" mapping.  The
         # descriptors here keep the materials' constants: the texture tables come from the host (read_dump_textures)
         self.texture_specs = {k: dict(v) for k, v in (textures or {}).items()}
+        # alpha masks: {material name (its meshes and objects) or "light" (the area-light quads): {"alpha" / "shadowalpha":
+        # 0 (written as "float alpha" [0]) or a mask spec {map: [h][w] texels (written as a PFM), wrap, trilinear,
+        # maxanisotropy, scale, uscale, vscale, udelta, vdelta}}}; write_pbrt declares the maps as float imagemap textures
+        # under the "uv" mapping.  The descriptors here carry no masks: their tables come from the host.
+        self.alpha_specs = {k: dict(v) for k, v in (alphas or {}).items()}
         self._lights = (abi.AreaLight * max(nl + len(self.delta_specs) + len(self.infinite_specs) + n_sl, 1))()
         for i in range(nl):
             self._lights[i].triangle = i
@@ -475,6 +480,32 @@ def _texture_lines(scene, name, dirname):
     return lines, mats
 
 
+def _alpha_lines(scene, name, dirname):
+    """The Texture statements of scene.alpha_specs (and their PFMs); {group: shape parameters naming its masks}."""
+    lines, params = [], {}
+    for group, kinds in sorted(getattr(scene, "alpha_specs", {}).items()):
+        p = ""
+        for kind, t in sorted(kinds.items()):
+            if not isinstance(t, dict):
+                p += ' "float %s" [%.9g]' % (kind, t)
+                continue
+            tex = "%s_%s" % (group, kind)
+            pfm = "%s_alpha_%s.pfm" % (name, tex)
+            m = np.asarray(t["map"], np.float32)
+            write_pfm(os.path.join(dirname, pfm), np.repeat(m[:, :, None], 3, axis=2) if m.ndim == 2 else m)
+            line = 'Texture "%s" "float" "imagemap" "string filename" "%s"' % (tex, pfm)
+            for key, k2 in (("wrap", "string"), ("trilinear", "bool"), ("maxanisotropy", "float"), ("scale", "float"),
+                            ("uscale", "float"), ("vscale", "float"), ("udelta", "float"), ("vdelta", "float")):
+                if key in t:
+                    v = t[key]
+                    line += ' "%s %s" [%s]' % (k2, key, ('"%s"' % v) if k2 == "string" else
+                                               ('"true"' if v else '"false"') if k2 == "bool" else "%.9g" % v)
+            lines.append(line)
+            p += ' "texture %s" "%s"' % (kind, tex)
+        params[group] = p
+    return lines, params
+
+
 def write_pbrt(dirname, name, scene, xres, yres, spp, max_depth=5, strategy="uniform", pixel_bounds=None,
                eye=(0, 0, -4.5), look=(0, 0, 0), up=(0, 1, 0), fov=35.0, lens_radius=0.0, focal_distance=1e6,
                crop_window=None, film_scale=1.0, max_sample_luminance=None, sampler="sobol", pixel_filter=None,
@@ -510,6 +541,8 @@ def write_pbrt(dirname, name, scene, xres, yres, spp, max_depth=5, strategy="uni
     tex_lines, tex_mats = _texture_lines(scene, name, dirname)
     lines += tex_lines
     material = lambda m: tex_mats.get(m, PBRT_MATERIAL[m])
+    alpha_lines, alpha_params = _alpha_lines(scene, name, dirname)
+    lines += alpha_lines
     for q in scene.light_quads:
         # quad() stores (p0 p1 p2)(p0 p2 p3); recover the 4 corners
         pts = [q[0][0], q[0][1], q[0][2], q[1][2]]
@@ -519,7 +552,7 @@ def write_pbrt(dirname, name, scene, xres, yres, spp, max_depth=5, strategy="uni
                   (scene.light_L, scene.light_L, scene.light_L,
                    ' "bool twosided" "true"' if scene.two_sided else ""),
                   '  Material "matte" "rgb Kd" [0 0 0]',
-                  '  Shape "trianglemesh" "integer indices" [0 1 2 0 2 3] "point P" [%s]' % flat,
+                  '  Shape "trianglemesh" "integer indices" [0 1 2 0 2 3] "point P" [%s]' % flat + alpha_params.get("light", ""),
                   "AttributeEnd"]
     for dl in getattr(scene, "delta_specs", ()):
         val = dl.get("I", dl.get("L", 1.0))
@@ -553,14 +586,15 @@ def write_pbrt(dirname, name, scene, xres, yres, spp, max_depth=5, strategy="uni
                   scene.uvs[sel] if m in scene.uv_meshes else None)
         if m in scene.reverse_orientation:
             lines += ["AttributeBegin", "ReverseOrientation"]
-        lines += [material(scene.material_names[m]), 'Shape "plymesh" "string filename" "%s"' % ply]
+        lines += [material(scene.material_names[m]),
+                  'Shape "plymesh" "string filename" "%s"' % ply + alpha_params.get(scene.material_names[m], "")]
         if m in scene.reverse_orientation:
             lines += ["AttributeEnd"]
     for k, (o, part) in enumerate(zip(getattr(scene, "object_specs", ()), getattr(scene, "object_parts", ()))):
         ply = "%s_obj%d.ply" % (name, k)
         write_ply(os.path.join(dirname, ply), part)
         lines += ['ObjectBegin "obj%d"' % k, "  " + material(o.get("material", "matte")),
-                  '  Shape "plymesh" "string filename" "%s"' % ply, "ObjectEnd"]
+                  '  Shape "plymesh" "string filename" "%s"' % ply + alpha_params.get(o.get("material", "matte"), ""), "ObjectEnd"]
     for ins in getattr(scene, "instance_specs", ()):
         lines.append("AttributeBegin")
         lines += ["  %s %s" % (op, " ".join("%.9g" % v for v in args)) for op, args in instance_steps(ins)]
@@ -599,6 +633,13 @@ def read_dump_infinite(path, abi):
     return _read_dump_tail(path, abi)[0]
 
 
+def read_dump_alpha(path, abi):
+    """(masks, alpha ids, shadowalpha ids) of the alpha masks an RGBSpectrum host wrote to its B200PT_DUMP_SCENE file
+    (behind the texture tables): masks are dicts {texels ([h][w] array, None for a constant 0), wrap, su, sv, du, dv}
+    for Scene.add_alpha_mask, the ids one per triangle for Scene.set_alpha_masks; ([], None, None) without masks."""
+    return _read_dump_tail(path, abi)[2]
+
+
 def read_dump_textures(path, abi):
     """(mipmaps, binds) of the image textures an RGBSpectrum host wrote to its B200PT_DUMP_SCENE file (behind the infinite
     lights' tables): mipmaps are dicts {levels ([h][w][3] or [h][w] arrays), wrap, trilinear, max_anisotropy, weight_lut}
@@ -607,6 +648,7 @@ def read_dump_textures(path, abi):
 
 
 TEXTURE_MARKER = -2  # host/gpupath.cpp: the image textures' tables follow the infinite lights' behind this int32
+ALPHA_MARKER = -3  # ... and the alpha masks' tables follow those behind this one
 
 
 def _read_dump_tail(path, abi):
@@ -632,13 +674,14 @@ def _read_dump_tail(path, abi):
         a = [int(x) for x in np.frombuffer(raw, np.int32, n, off)]
         off += 4 * n
         return a
-    while off < len(raw) and int(np.frombuffer(raw, np.int32, 1, off)[0]) != TEXTURE_MARKER:
+    marker = lambda: int(np.frombuffer(raw, np.int32, 1, off)[0]) if off < len(raw) else None
+    while off < len(raw) and marker() not in (TEXTURE_MARKER, ALPHA_MARKER):
         light, w, h, nu, nv = ints(5)
         out[light] = dict(texels=take(w * h * 3, (h, w, 3)), light_to_world=take(16), cond_func=take(nv * nu, (nv, nu)),
                           cond_cdf=take(nv * (nu + 1), (nv, nu + 1)), cond_func_int=take(nv), marg_func=take(nv),
                           marg_cdf=take(nv + 1), marg_func_int=take(1)[0], power_rgb=take(3))
     mips, binds = [], []
-    if off < len(raw):
+    if marker() == TEXTURE_MARKER:
         _, nmip, nbind = ints(3)
         for _ in range(nmip):
             nlev, ch, wrap, tri = ints(4)
@@ -653,9 +696,17 @@ def _read_dump_tail(path, abi):
             mat, slot, mip = ints(3)
             su, sv, du, dv = (float(x) for x in take(4))
             binds.append(dict(material=mat, slot=slot, mipmap=mip, su=su, sv=sv, du=du, dv=dv, remap=ints(1)[0]))
+    masks, alpha, shadow = [], None, None
+    if marker() == ALPHA_MARKER:
+        _, nmask = ints(2)
+        for _ in range(nmask):
+            w, h, wrap = ints(3)
+            su, sv, du, dv = (float(x) for x in take(4))
+            masks.append(dict(texels=take(w * h, (h, w)) if w else None, wrap=wrap, su=su, sv=sv, du=du, dv=dv))
+        alpha, shadow = np.array(ints(nt), np.int32), np.array(ints(nt), np.int32)
     if off != len(raw):
-        raise ValueError("%s: truncated infinite-light or texture tables" % path)
-    return out, (mips, binds)
+        raise ValueError("%s: truncated infinite-light, texture or alpha-mask tables" % path)
+    return out, (mips, binds), (masks, alpha, shadow)
 
 
 def read_pfm(path):
