@@ -167,7 +167,11 @@ static TravBounds make_trav_bounds(const float *lo, const float *hi) {
     b.scale = std::max(absmax, ext);
     return b;
 }
-// the tree-related members of a traversal launch
+static int sphere_refill_lanes() {
+    static int v = getenv("B200PT_SPHERE_REFILL") ? atoi(getenv("B200PT_SPHERE_REFILL")) : 8;
+    return v;
+}
+// the scene's members of a traversal launch: its trees, alpha masks, spheres and instances
 static void trace_args_scene(TraceArgs &a, const b200pt_scene *s) {
     a.nodes = s->d_nodes;
     a.tri_base = s->d_tri_base;
@@ -179,6 +183,14 @@ static void trace_args_scene(TraceArgs &a, const b200pt_scene *s) {
     a.alpha_ids = s->d_alpha_ids;
     a.tri_uv = s->d_tri_uv;
     a.alpha_any_shadow = 1;
+    a.spheres = s->d_spheres;
+    a.n_spheres = (uint32_t)s->spheres.size();
+    a.n_tris = (uint32_t)s->n_prims;
+    a.sphere_refill_lanes = sphere_refill_lanes();
+    a.instances = s->d_instances;
+    a.n_instances = (uint32_t)s->instances.size();
+    a.tlas_node_off = s->tlas_node_off;
+    a.tlas_tri_off = s->tlas_tri_off;
 }
 // the members every traversal launch of a render shares: the tree's, plus the per-slot record stride and the k_trace knobs;
 // everything else zero
@@ -993,10 +1005,6 @@ static int refill_lanes() {
     static int v = getenv("B200PT_REFILL_LANES") ? atoi(getenv("B200PT_REFILL_LANES")) : 26;
     return v;
 }
-static int sphere_refill_lanes() {
-    static int v = getenv("B200PT_SPHERE_REFILL") ? atoi(getenv("B200PT_SPHERE_REFILL")) : 8;
-    return v;
-}
 
 // Scenes with object instances: the persistent two-level kernel (k_trace2) walks top-level triangles and instances in
 // one launch.  Scenes that also hold Sphere shapes (tested by the separate pass k_spheres, which needs every earlier hit's
@@ -1009,6 +1017,30 @@ static bool two_level(const b200pt_scene *s) {
     static const bool off = getenv("B200PT_NO_TRACE2") != nullptr;
     return !off && !s->instances.empty() && s->tlas_node_off != 0 && s->spheres.empty();
 #endif
+}
+
+// Scene::Intersect / IntersectP of the rays in `a` (trace_args_scene filled its scene members): the traversal launch and,
+// when the scene has shapes that launch does not test (spheres; instances outside the two-level kernel), the pass over
+// those (fetch counter sphere_work).  With `classify` the hits go to their BSDF family's queue: by the sphere pass when
+// it runs, since it decides the final hit.  `count` (instrumented renders) runs the single-level kernel, which counts
+// node and triangle tests.  hit_inst_out: where closest hits on object triangles leave their instance, or nullptr.
+// Returns true when the sphere pass was launched (the traversal launch is always one).
+static bool scene_intersect(const b200pt_scene *s, TraceArgs a, bool any_hit, bool classify, bool count, int grid_trace,
+                            int grid_spheres, uint32_t *sphere_work, uint32_t *hit_inst_out, cudaStream_t st) {
+    const bool tl = two_level(s) && !count;
+    const bool spheres = a.n_spheres > 0 || (a.n_instances > 0 && !tl);
+    a.hit_inst_out = hit_inst_out;
+    a.sphere_work = sphere_work;
+#ifndef B200PT_HOST_EMU
+    if (tl)
+        launch_trace2(a, any_hit, classify && !spheres, grid_trace, st);
+    else
+#endif
+        launch_trace(a, any_hit, classify && !spheres, count, grid_trace, st);
+    if (!spheres) return false;
+    if (tl) a.n_instances = 0;  // already walked
+    launch_spheres(a, any_hit, classify, grid_spheres, st);
+    return true;
 }
 
 static int trace_dev(b200pt_scene *s, uint64_t rays_dev, uint64_t out_dev, int64_t n, bool any_hit) {
@@ -1037,26 +1069,7 @@ static int trace_dev(b200pt_scene *s, uint64_t rays_dev, uint64_t out_dev, int64
         a.occ_out = reinterpret_cast<uint8_t *>(out_dev);
     else
         a.full_out = reinterpret_cast<b200pt_hit *>(out_dev);
-    const bool tl = two_level(s);
-    a.spheres = s->d_spheres;
-    a.n_spheres = (uint32_t)s->spheres.size();
-    a.instances = s->d_instances;
-    a.n_instances = (uint32_t)s->instances.size();
-    a.tlas_node_off = s->tlas_node_off;
-    a.tlas_tri_off = s->tlas_tri_off;
-    a.n_tris = (uint32_t)s->n_prims;
-    a.sphere_work = s->d_work + 2;
-    a.sphere_refill_lanes = sphere_refill_lanes();
-#ifndef B200PT_HOST_EMU
-    if (tl)
-        launch_trace2(a, any_hit, false, trace_grid(s->ctx), st);
-    else
-#endif
-        launch_trace(a, any_hit, false, false, trace_grid(s->ctx), st);
-    if (!s->spheres.empty() || (!s->instances.empty() && !tl)) {
-        if (tl) a.n_instances = 0;  // already walked
-        launch_spheres(a, any_hit, false, trace_grid(s->ctx), st);
-    }
+    scene_intersect(s, a, any_hit, false, false, trace_grid(s->ctx), trace_grid(s->ctx), s->d_work + 2, nullptr, st);
     CUDA_TRY(cudaGetLastError());
     return B200PT_OK;
 }
@@ -1801,9 +1814,7 @@ int b200pt_render_tiles(b200pt_render *r, const int32_t *tiles, int64_t n_tiles)
         };
         const bool overlap = r->overlap && !medium;
         cudaStream_t st2 = overlap ? ctx->stream_aux : st;
-        const bool tl = two_level(r->scene) && !r->instrumented;  // instances inside the traversal kernel
-        const bool has_spheres = H.scene.n_spheres > 0 || (H.scene.n_instances > 0 && !tl);  // "extra shapes" pass needed
-        const bool full_shade = has_spheres || H.scene.n_instances > 0 || H.has_delta_lights || H.scene.tri_n != nullptr ||
+        const bool full_shade = H.scene.n_spheres > 0 || H.scene.n_instances > 0 || H.has_delta_lights || H.scene.tri_n != nullptr ||
                                 H.scene.tri_uv != nullptr || H.volpath || H.n_infinite > 0 || H.tex_bind != nullptr;
         // escaped path rays of bounce b (scenes with infinite lights, RGB build only): after resolve(b - 1), before shade(b + 1)
         // rewrites the bounce's path queue
@@ -1812,39 +1823,11 @@ int b200pt_render_tiles(b200pt_render *r, const int32_t *tiles, int64_t n_tiles)
             LaunchTimer lt(r, st, 2);
             launch_escape(r->d_dev, b, H.work + (size_t)b * W_PER_BOUNCE + W_ESCAPE, r->grid_shade, st);
         };
-        // traversal of one ray queue: the plain kernel, or the two-level one when the scene has instances
-        auto trace = [&](TraceArgs &a, bool any_hit, bool classify, cudaStream_t s_) {
-#ifndef B200PT_HOST_EMU
-            if (tl) {
-                a.instances = H.scene.instances;
-                a.n_instances = H.scene.n_instances;
-                a.tlas_node_off = H.scene.tlas_node_off;
-                a.tlas_tri_off = H.scene.tlas_tri_off;
-                a.hit_inst_out = a.hit_out == &H.path->hit ? &H.path->hit_inst : nullptr;
-                launch_trace2(a, any_hit, classify, r->grid_trace, s_);
-                return;
-            }
-#endif
-            launch_trace(a, any_hit, classify, r->instrumented, r->grid_trace, s_);
-        };
-        // Scene::Intersect / IntersectP of the ray queue in `a`: the traversal launch and, with `spheres`, the pass over the
-        // shapes outside the tree (fetch counter sphere_work).  With `classify` the hits go to their BSDF family's queue:
-        // by the sphere pass when it runs, since it decides the final hit.
-        auto intersect = [&](TraceArgs &a, bool any_hit, bool classify, bool spheres, uint32_t *sphere_work, cudaStream_t s_) {
-            trace(a, any_hit, classify && !spheres, s_);
-            if (!spheres) return;
-            a.sphere_refill_lanes = sphere_refill_lanes();
-            a.spheres = H.scene.spheres;
-            a.n_spheres = H.scene.n_spheres;
-            a.instances = H.scene.instances;
-            a.n_instances = tl ? 0u : H.scene.n_instances;
-            a.tlas_node_off = H.scene.tlas_node_off;
-            a.tlas_tri_off = H.scene.tlas_tri_off;
-            a.hit_inst_out = a.hit_out == &H.path->hit ? &H.path->hit_inst : nullptr;
-            a.n_tris = (uint32_t)r->scene->n_prims;
-            a.sphere_work = sphere_work;
-            launch_spheres(a, any_hit, classify, r->grid_shade, s_);
-            r->launches++;
+        // Scene::Intersect / IntersectP of the ray queue in `a` (scene_intersect); path rays keep the instance of their hit
+        auto intersect = [&](const TraceArgs &a, bool any_hit, bool classify, uint32_t *sphere_work, cudaStream_t s_) {
+            uint32_t *hit_inst = a.hit_out == &H.path->hit ? &H.path->hit_inst : nullptr;
+            if (scene_intersect(r->scene, a, any_hit, classify, r->instrumented, r->grid_trace, r->grid_shade, sphere_work, hit_inst, s_))
+                r->launches++;
         };
         auto trace_path = [&](int b) {
             uint32_t *qc = H.qcount + (size_t)b * Q_PER_BOUNCE;
@@ -1866,7 +1849,7 @@ int b200pt_render_tiles(b200pt_render *r, const int32_t *tiles, int64_t n_tiles)
                 // the medium pass below is timed on its own (category 2)
                 LaunchTimer lt(r, st, 0);
                 // inside a medium the medium pass classifies (only paths that reach their surface are shaded)
-                intersect(a, false, !medium, has_spheres, wk + W_SPHERES_PATH, st);
+                intersect(a, false, !medium, wk + W_SPHERES_PATH, st);
             }
             if (general) {
                 // the medium pass, then -- while some rays reached a medium boundary -- the same two steps again for those
@@ -1884,7 +1867,7 @@ int b200pt_render_tiles(b200pt_render *r, const int32_t *tiles, int64_t n_tiles)
                     a.work = wc + WC_TRACE;
                     {
                         LaunchTimer lt(r, st, 0);
-                        intersect(a, false, false, true, wc + WC_SPHERES, st);
+                        intersect(a, false, false, wc + WC_SPHERES, st);
                     }
                     LaunchTimer lt2(r, st, 2);
                     launch_medium_general(r->d_dev, H, b, H.q_cross[cur], wc + cur, cur ^ 1, wc + (cur ^ 1), wc + WC_WALK, true, r->grid_shade,
@@ -1925,7 +1908,7 @@ int b200pt_render_tiles(b200pt_render *r, const int32_t *tiles, int64_t n_tiles)
                 a.work = trace_work;
                 {
                     LaunchTimer lt(r, st, 0);
-                    intersect(a, false, false, true, sphere_work, st);
+                    intersect(a, false, false, sphere_work, st);
                 }
                 {
                     LaunchTimer lt2(r, st, 2);
@@ -1956,7 +1939,7 @@ int b200pt_render_tiles(b200pt_render *r, const int32_t *tiles, int64_t n_tiles)
             a.occ_out = &H.direct->occluded;
             {
                 LaunchTimer lt(r, st2, 1);
-                intersect(a, true, false, has_spheres, wk + W_SPHERES_SHADOW, st2);
+                intersect(a, true, false, wk + W_SPHERES_SHADOW, st2);
             }
             // BSDF-sampled MIS rays (closest hit)
             a.ray_o = &H.direct->mi_o;
@@ -1968,7 +1951,7 @@ int b200pt_render_tiles(b200pt_render *r, const int32_t *tiles, int64_t n_tiles)
             a.hit_out = &H.direct->mis_hit;
             a.occ_out = nullptr;
             LaunchTimer lt(r, st2, 0);
-            intersect(a, false, false, has_spheres, wk + W_SPHERES_MIS, st2);
+            intersect(a, false, false, wk + W_SPHERES_MIS, st2);
         };
         trace_path(0);
         escape(0);

@@ -260,8 +260,8 @@ __global__ void __launch_bounds__(256) k_raygen_pfilm(const RenderDev *R, uint32
 // still traversing (TraceArgs::refill_lanes); then the warp reconverges, finished rays are written out
 // (+ classified by BSDF family with warp-aggregated appends) and idle lanes
 // fetch new rays -- so one long ray never keeps 31 lanes idle.
-// Every traversal kernel has a twin k_*_alpha for scenes with alpha masks (AlphaTest); scenes without masks launch
-// the plain kernels.
+// Every traversal kernel takes the mask test as its class ALPHA: AlphaTest for scenes with alpha masks, NoAlpha
+// (wbvh_traverse.cuh) for the rest; the launchers pick it from TraceArgs::alpha_masks.
 
 // Alpha masks inside intersection (Triangle::Intersect / IntersectP, shapes/triangle.cpp:332-337, 531-570): a candidate
 // the watertight test accepted is rejected when a mask of its mesh evaluates to exactly 0 at uvHit = b0 uv0 + b1 uv1 +
@@ -430,6 +430,36 @@ __device__ __forceinline__ void ray_store_hit(float *col, const TravRay &R) {
     col[12 * 128] = R.hit.b2;
 }
 
+// Writes out the lane's ray if it is finished (`fin`; its record is the column my_ray, its stack state sp) and, with
+// CLASSIFY, appends its slot to the queue of the hit's BSDF family.  hit_inst (k_trace2): where the instance of a hit
+// goes (record word 21), or nullptr.  Every lane of the warp must call it (converged).
+template <bool ANY_HIT, bool CLASSIFY>
+__device__ __forceinline__ void retire_ray(const TraceArgs &a, const float *my_ray, bool fin, uint32_t slot, uint32_t sp,
+                                           uint32_t *hit_inst) {
+    int family = -1;
+    if (fin) {
+        const uint32_t best = __float_as_uint(my_ray[8 * 128]);
+        if (ANY_HIT) {
+            slot_out(a.occ_out, slot, a.out_stride) = best != B200PT_MISS ? 1 : 0;
+        } else {
+            if (a.hit_out) slot_out(a.hit_out, slot, a.out_stride) = best;
+            if (hit_inst && best != B200PT_MISS) slot_out(hit_inst, slot, a.out_stride) = __float_as_uint(my_ray[21 * 128]);
+            if (a.full_out) {
+                b200pt_hit r;
+                r.triangle = best != B200PT_MISS ? (int32_t)__float_as_uint(ld_f4(a.tris + (size_t)best * 3).w) : -1;
+                r.t = my_ray[9 * 128];
+                r.b0 = my_ray[10 * 128];
+                r.b1 = my_ray[11 * 128];
+                a.full_out[slot] = r;
+            }
+            if (CLASSIFY && best != B200PT_MISS)
+                family = hit_family(a.materials, __float_as_uint(ld_f4(a.tris + (size_t)best * 3 + 1).w));
+        }
+        if ((sp & B200PT_SP_OVERFLOW) && a.stats) atomicAdd(&a.stats[7], 1ull);
+    }
+    if (CLASSIFY) append_family(a.q_mat, a.qcount_mat, family, slot);
+}
+
 template <bool ANY_HIT, bool CLASSIFY, bool COUNT, class ALPHA>
 __device__ __forceinline__ void trace_walk(const TraceArgs a, const ALPHA alpha) {
     // the slot-permutation table of the node test (wbvh_traverse.cuh), one copy per CTA
@@ -439,7 +469,6 @@ __device__ __forceinline__ void trace_walk(const TraceArgs a, const ALPHA alpha)
     __syncthreads();
     float *const my_ray = s_ray + threadIdx.x;
     const uint32_t n = *a.count;
-    const int lane = threadIdx.x & 31;
     TraceCounters ctr;
     ctr.nodes = ctr.tris = 0;
     Trav T;
@@ -448,35 +477,16 @@ __device__ __forceinline__ void trace_walk(const TraceArgs a, const ALPHA alpha)
     bool has = false, fin = false, exhausted = false;
     while (true) {
         // ---- converged: retire finished rays
-        {
-            int family = -1;
-            if (fin) {
-                const uint32_t best = __float_as_uint(my_ray[8 * 128]);
-                if (ANY_HIT) {
-                    slot_out(a.occ_out, slot, a.out_stride) = best != B200PT_MISS ? 1 : 0;
-                } else {
-                    if (a.hit_out) slot_out(a.hit_out, slot, a.out_stride) = best;
-                    if (a.full_out) {
-                        b200pt_hit r;
-                        r.triangle = best != B200PT_MISS ? (int32_t)__float_as_uint(ld_f4(a.tris + (size_t)best * 3).w) : -1;
-                        r.t = my_ray[9 * 128];
-                        r.b0 = my_ray[10 * 128];
-                        r.b1 = my_ray[11 * 128];
-                        a.full_out[slot] = r;
-                    }
-                    if (CLASSIFY && best != B200PT_MISS)
-                        family = hit_family(a.materials, __float_as_uint(ld_f4(a.tris + (size_t)best * 3 + 1).w));
-                }
-                if ((T.sp & B200PT_SP_OVERFLOW) && a.stats) atomicAdd(&a.stats[7], 1ull);
-            }
-            if (CLASSIFY) append_family(a.q_mat, a.qcount_mat, family, slot);
-            fin = false;
-        }
-        // ---- converged: idle lanes fetch new rays
+        retire_ray<ANY_HIT, CLASSIFY>(a, my_ray, fin, slot, T.sp, nullptr);
+        fin = false;
+        // ---- converged: idle lanes fetch new rays.  warp_append written out: through warp_append this kernel
+        // compiles to another schedule, and cfg4 took 8042 and 8044 ms per step against 8030 and 8030 written out
+        // (bench.py, the two builds alternating, H100 80GB HBM3 at 700 W)
         {
             const bool want = !has && !exhausted;
             const uint32_t mask = __ballot_sync(FULL_MASK, want);
             if (mask) {
+                const int lane = threadIdx.x & 31;
                 const int leader = __ffs(mask) - 1;
                 uint32_t base = 0;
                 if (lane == leader) base = atomicAdd(a.work, (uint32_t)__popc(mask));
@@ -577,56 +587,521 @@ __device__ __forceinline__ void trace_walk(const TraceArgs a, const ALPHA alpha)
 // one-batch-of-32-rays walk of k_spheres for the instances.
 #define B200PT_RAY_WORDS2 24  // k_trace's record + 21 instance of the hit, 22 world tMax, 23 current instance
 #define B200PT_MARK 0x80000000u  // stack entry x: "what follows is what the lane left behind when it entered an instance"
-#define B200PT_WALK(x) x
-#define B200PT_WALK_ALPHA(off)
-#include "trace2_kernel.cuh"
-#undef B200PT_WALK
-#undef B200PT_WALK_ALPHA
-#define B200PT_WALK(x) x##_alpha
-#define B200PT_WALK_ALPHA(off) , AlphaTest::of(a).at(off)
-#include "trace2_kernel.cuh"
-#undef B200PT_WALK
-#undef B200PT_WALK_ALPHA
+template <bool ANY_HIT, bool CLASSIFY, class ALPHA>
+__global__ void __launch_bounds__(128, 6) k_trace2(const TraceArgs a) {
+    __shared__ __align__(16) uint8_t s_lut[B200PT_LUT_BYTES];
+    __shared__ float s_ray[B200PT_RAY_WORDS2 * 128];
+    reinterpret_cast<uint4 *>(s_lut)[threadIdx.x] = __ldg(reinterpret_cast<const uint4 *>(a.lut) + threadIdx.x);
+    __syncthreads();
+    float *const my_ray = s_ray + threadIdx.x;
+    const uint32_t n = *a.count;
+    TraceCounters ctr;
+    ctr.nodes = ctr.tris = 0;
+    Trav T;
+    TravStack S;
+    uint32_t slot = 0, pend_x = 0, pend_y = 0;
+    uint32_t noff = 0, toff = 0;  // the tree the lane is in: offsets of its nodes / triangles inside the scene's arrays
+    int phase = 0;                // 0: top-level tree, 1: tree over the instances, 2: inside an instance
+    bool has = false, fin = false, exhausted = false;
+    bool want_exit = false;       // the object's tree is exhausted: the lane waits to go back to the world ray
+    // (re)derives the box-test constants and the triangle-test record for a ray in the space the lane enters;
+    // the position on the stack and the result so far are the lane's own and stay
+    auto enter_space = [&](const V3 &o, const V3 &d, float tmax, const TravBounds &B) {
+        TravRay R;
+        const int sp = T.sp;
+        trav_init(T, R, o, d, tmax, B);
+        T.sp = sp;
+        my_ray[0 * 128] = R.o.x;
+        my_ray[1 * 128] = R.o.y;
+        my_ray[2 * 128] = R.o.z;
+        my_ray[3 * 128] = R.sh.Sx;
+        my_ray[4 * 128] = R.sh.Sy;
+        my_ray[5 * 128] = R.sh.Sz;
+        my_ray[6 * 128] = __int_as_float(R.sh.kz);
+        my_ray[7 * 128] = R.tmax;
+        my_ray[13 * 128] = R.t0;
+        my_ray[14 * 128] = R.iu[0];
+        my_ray[15 * 128] = R.iu[1];
+        my_ray[16 * 128] = R.iu[2];
+        my_ray[17 * 128] = R.ou[0];
+        my_ray[18 * 128] = R.ou[1];
+        my_ray[19 * 128] = R.ou[2];
+        my_ray[20 * 128] = R.span_floor;
+    };
+    auto world_ray = [&](V3 *o, V3 *d) {
+        const float4 o4 = a.ray_o[(size_t)slot * a.stride];
+        const float4 d4 = a.ray_d[(size_t)slot * a.stride];
+        *o = v3(o4);
+        *d = v3(d4);
+    };
+    while (true) {
+        // ---- converged: retire finished rays
+        retire_ray<ANY_HIT, CLASSIFY>(a, my_ray, fin, slot, T.sp, a.hit_inst_out);
+        fin = false;
+        // ---- converged: idle lanes fetch new rays
+        {
+            const bool want = !has && !exhausted;
+            const uint32_t i = warp_append(a.work, want);
+            if (want) {
+                if (i < n) {
+                    slot = a.queue ? a.queue[i] : i;
+                    const float4 o4 = a.ray_o[(size_t)slot * a.stride];
+                    const float4 d4 = a.ray_d[(size_t)slot * a.stride];
+                    const float tmax = a.t_max_from_w ? o4.w : a.fixed_t_max;
+                    T.sp = 0;
+                    phase = 0;
+                    want_exit = false;
+                    noff = toff = 0;
+                    enter_space(v3(o4), v3(d4), tmax, a.bounds);
+                    my_ray[8 * 128] = __uint_as_float(B200PT_MISS);
+                    my_ray[9 * 128] = my_ray[10 * 128] = my_ray[11 * 128] = my_ray[12 * 128] = 0.f;
+                    my_ray[21 * 128] = __uint_as_float(0u);
+                    my_ray[22 * 128] = tmax;  // the world ray's tMax
+                    pend_y = 0;
+                    has = true;
+                } else {
+                    exhausted = true;
+                }
+            }
+        }
+        if (__ballot_sync(FULL_MASK, has) == 0) break;
+        while (has) {
+            uint32_t ng_x = 0, ng_y = 0;
+            // Entering an instance leaves ONE group of untried candidates behind, so in the tree over the instances a lane
+            // holds (takes no node step) while it has a leaf group; a lane that is done with an object's tree waits the
+            // same way.  Both wait for company: changing space is ~900 instructions and runs once the usual share of the
+            // warp's lanes has something parked (triangles, candidates, a way back), not one lane at a time.
+            const bool hold = (phase == 1 && pend_y != 0) || want_exit;
+            const bool node_work = !hold && (T.cur_y & 0xff000000u) != 0;
+            if (node_work)
+                trav_node_phase<!ANY_HIT, false>(T, S, a.nodes + (size_t)noff * 4, a.tri_base + noff, s_lut, &ng_x, &ng_y, &ctr);
+            bool must = false;
+            if (ng_y) {
+                if (pend_y) {
+                    must = true;  // two groups: flush the parked one now, park the new one after
+                } else {
+                    pend_x = ng_x;
+                    pend_y = ng_y;
+                    ng_y = 0;
+                }
+            }
+            const bool out_of_nodes = (T.cur_y & 0xff000000u) == 0;  // (what is left on the stack waits behind the parked group)
+            const unsigned act = __activemask();
+            const bool parked_me = pend_y != 0 || want_exit;
+            const bool idle_me = hold || (phase == 1 && pend_y != 0) || (out_of_nodes && pend_y != 0);
+            const unsigned counts = __reduce_add_sync(
+                act, (parked_me ? 1u : 0u) | ((must || (idle_me && a.postpone_pct <= 0)) ? 0x100u : 0u) | (idle_me ? 0x10000u : 0u));
+            const int n_act = __popc(act), n_parked = (int)(counts & 0xffu), n_idle = (int)((counts >> 16) & 0xffu);
+            if ((counts & 0xff00u) || n_parked * 100 >= n_act * a.postpone_pct || n_idle * 4 >= n_act) {
+                bool done = false;
+                if (want_exit) {
+                    // the object's tree is done: back to the world ray (its tMax is the hit's, if there was one) and to
+                    // the walk over the instances -- first the candidates of the same leaf that were not tried
+                    want_exit = false;
+                    uint32_t ex, ey, gx, gy;
+                    T.sp -= 2;
+                    S.pop((T.sp & B200PT_SP_MASK) + 1, &ex, &ey);
+                    S.pop(T.sp & B200PT_SP_MASK, &gx, &gy);
+                    V3 ro, rd;
+                    world_ray(&ro, &rd);
+                    noff = a.tlas_node_off;
+                    toff = a.tlas_tri_off;
+                    phase = 1;
+                    enter_space(ro, rd, my_ray[22 * 128], a.tlas_bounds);
+                    T.cur_x = gx;
+                    T.cur_y = gy;
+                    if (ey) {
+                        pend_x = ex;  // marked: already a triangle group
+                        pend_y = ey;
+                    }
+                } else if (pend_y && phase == 1) {
+                    // leaf of the tree over the instances: its "triangles" name instances; the first candidate whose
+                    // leaf box the ray (with its current tMax) enters takes the lane into that object's tree
+                    uint32_t tg_x, tg_y;
+                    if (pend_x & B200PT_MARK) {  // candidates left over from before an instance was entered: already triangles
+                        tg_x = pend_x & ~B200PT_MARK;
+                        tg_y = pend_y;
+                    } else {
+                        leaf_group_triangles(a.tri_base + noff, pend_x, pend_y, &tg_x, &tg_y);
+                    }
+                    pend_y = 0;
+                    V3 ro, rd;
+                    world_ray(&ro, &rd);
+                    const float wtmax = my_ray[22 * 128];
+                    while (tg_y) {
+                        const int j = msb32(tg_y);
+                        tg_y &= ~(1u << j);
+                        const uint32_t k = __float_as_uint(ld_f4(a.tris + (size_t)(toff + tg_x + (uint32_t)j) * 3).w);  // TriRecord::prim
+                        const DevInstance &in = a.instances[k];
+                        if (!instance_leaf_test(in, ro, rd, wtmax)) continue;
+                        // left behind: the group being walked and the candidates not tried yet
+                        if ((T.sp & B200PT_SP_MASK) + 2 > B200PT_STACK) {
+                            T.sp |= B200PT_SP_OVERFLOW;
+                            break;
+                        }
+                        S.push(T.sp & B200PT_SP_MASK, T.cur_x, T.cur_y);
+                        S.push((T.sp & B200PT_SP_MASK) + 1, tg_x | B200PT_MARK, tg_y);
+                        T.sp += 2;
+                        V3 o2, d2;
+                        float tm2;
+                        instance_ray(in, ro, rd, wtmax, &o2, &d2, &tm2);
+                        enter_space(o2, d2, tm2, instance_bounds(in));
+                        noff = in.node_off;
+                        toff = in.tri_off;
+                        my_ray[23 * 128] = __uint_as_float(k);
+                        phase = 2;
+                        break;
+                    }
+                } else if (pend_y) {
+                    TravRay R;
+                    ray_load(my_ray, R);
+                    R.best = B200PT_MISS;  // (an index inside this tree; the record keeps scene-wide ones)
+                    done = trav_tri_phase<ANY_HIT, false>(R, a.tri_base + noff, a.tris + (size_t)toff * 3, pend_x, pend_y, &ctr, ALPHA::of(a).at(toff));
+                    if (R.best != B200PT_MISS) {
+                        R.best += toff;
+                        ray_store_hit(my_ray, R);
+                        if (!ANY_HIT) {
+                            ray_load_scale(my_ray, R);
+                            trav_rescale(T, R, R.tmax);
+                        }
+                        if (phase == 2) my_ray[21 * 128] = my_ray[23 * 128];  // the instance of the hit
+                        my_ray[22 * 128] = R.tmax;                            // r.tMax = ray.tMax (primitive.cpp:91 / :120)
+                    }
+                    pend_y = 0;
+                }
+                if (ng_y) {  // the second group found in this step (only outside the tree over the instances)
+                    pend_x = ng_x;
+                    pend_y = ng_y;
+                }
+                if (done) {
+                    has = false;
+                    fin = true;
+                    pend_y = 0;
+                }
+            }
+            // ---- the next group of the current tree, or (later, in company) back out of an instance, or on to the next tree, or done
+            if (has && !want_exit && (T.cur_y & 0xff000000u) == 0) {
+                bool more = false, blocked = false;
+                while (!more && !blocked) {
+                    if ((T.sp & B200PT_SP_MASK) == 0) break;
+                    uint32_t ex, ey;
+                    S.pop((T.sp & B200PT_SP_MASK) - 1, &ex, &ey);
+                    if (!(ex & B200PT_MARK)) {
+                        --T.sp;
+                        T.cur_x = ex;
+                        T.cur_y = ey;
+                        more = (ey & 0xff000000u) != 0;
+                    } else {
+                        blocked = true;  // an object's tree is exhausted: leave it once its parked triangles are tested
+                        if (pend_y == 0) want_exit = true;
+                    }
+                }
+                if (!more && !blocked && pend_y == 0) {
+                    if (phase == 0 && a.n_instances > 0) {
+                        // the top-level triangles are done: on to the instances, with the ray's tMax so far
+                        V3 ro, rd;
+                        world_ray(&ro, &rd);
+                        noff = a.tlas_node_off;
+                        toff = a.tlas_tri_off;
+                        phase = 1;
+                        enter_space(ro, rd, my_ray[22 * 128], a.tlas_bounds);
+                        if ((T.cur_y & 0xff000000u) == 0) {
+                            has = false;
+                            fin = true;
+                        }
+                    } else {
+                        has = false;
+                        fin = true;
+                    }
+                }
+            }
+            if (__popc(__activemask()) < a.refill_lanes) break;
+        }
+        __syncwarp();
+    }
+}
 #endif  // B200PT_HOST_EMU
 
-template <bool ANY_HIT, bool CLASSIFY, bool COUNT>
+template <bool ANY_HIT, bool CLASSIFY, bool COUNT, class ALPHA>
 __global__ void __launch_bounds__(128, B200PT_TRACE_CTAS) k_trace(const TraceArgs a) {
-    trace_walk<ANY_HIT, CLASSIFY, COUNT>(a, NoAlpha());
-}
-template <bool ANY_HIT, bool CLASSIFY, bool COUNT>
-__global__ void __launch_bounds__(128, B200PT_TRACE_CTAS) k_trace_alpha(const TraceArgs a) {
-    trace_walk<ANY_HIT, CLASSIFY, COUNT>(a, AlphaTest::of(a));
+    trace_walk<ANY_HIT, CLASSIFY, COUNT>(a, ALPHA::of(a));
 }
 
 // ---------------------------------------------------------------------- instances
-// TransformedPrimitive::Intersect / IntersectP (primitive.cpp:76-106) for one instance with the current ray.tMax:
-// leaf-box gate, ray into the object's space, the object's own tree.  Closest: returns the triangle (index inside the
-// scene's leaf-order array) or B200PT_MISS and the hit; any-hit: B200PT_MISS or anything else.
-template <bool ANY_HIT>
-__device__ uint32_t instance_test(const TraceArgs &a, uint32_t k, const V3 &ro, const V3 &rd, float tmax, TriHit *h) {
-    const DevInstance &in = a.instances[k];
-    if (!instance_leaf_test(in, ro, rd, tmax)) return B200PT_MISS;
-    V3 o2, d2;
-    float tm2;
-    instance_ray(in, ro, rd, tmax, &o2, &d2, &tm2);
-    TraceCounters ctr;
-    uint32_t overflow = 0;
-    const uint32_t ti = traverse_wbvh<ANY_HIT, false>(a.nodes + (size_t)in.node_off * 4, a.tri_base + in.node_off,
-                                                      a.tris + (size_t)in.tri_off * 3, instance_bounds(in), a.lut, o2, d2, tm2, h, &ctr,
-                                                      &overflow);
-    if (overflow && a.stats) atomicAdd(&a.stats[7], (unsigned long long)overflow);
-    return ti == B200PT_MISS ? B200PT_MISS : in.tri_off + ti;
+// All instances against one ray, as a resumable state machine: through the tree over their leaf boxes when there is
+// one (its leaf "triangles" carry instance numbers), else one by one.  Each lane walks the tree over the instances'
+// boxes, picks the next candidate instance, or takes ONE step inside that instance's tree per call of step(), so that
+// the lanes of a warp meet again after every step instead of after whole nested traversals (measured with nested loops:
+// 2.4 of 32 lanes active per instruction) and a lane whose ray is done can take the next ray (k_spheres).
+template <bool ANY_HIT, class ALPHA>
+struct InstanceWalk {
+    Trav T1, T2;
+    TravRay R1, R2;
+    TravStack S1, S2;
+    V3 ro, rd;
+    uint32_t pend_x, pend_y, cur_inst, cur_tri_off, overflow;
+    const U4 *bn;
+    const uint32_t *bb;
+    const F4 *bt;
+    int state;  // 0: instance tree, 1: next candidate, 2: inside an instance, 3: done
+    uint32_t next_linear;  // scenes without a tree over the instances: the next instance to try
+    // results
+    uint32_t best, inst;
+    TriHit hit;
+
+    __device__ void init(const TraceArgs &a, const V3 &o, const V3 &d, float tmax) {
+        ro = o;
+        rd = d;
+        best = B200PT_MISS;
+        inst = 0;
+        hit.t = hit.b0 = hit.b1 = hit.b2 = 0.f;
+        pend_x = pend_y = cur_inst = cur_tri_off = overflow = 0;
+        next_linear = 0;
+        bn = nullptr;
+        bb = nullptr;
+        bt = nullptr;
+        state = 0;
+        trav_init(T1, R1, o, d, tmax, a.tlas_bounds);
+        if (a.tlas_node_off == 0u) {  // no tree: T1 only carries the ray's tMax
+            T1.cur_y = 0u;
+            R1.tmax = tmax;
+            state = 1;
+        }
+        T2 = T1;
+        R2 = R1;
+        T2.cur_y = 0u;
+    }
+    __device__ float tmax() const { return R1.tmax; }
+    __device__ bool enter(const TraceArgs &a, uint32_t k) {
+        const DevInstance &in = a.instances[k];
+        if (!instance_leaf_test(in, ro, rd, R1.tmax)) return false;
+        V3 o2, d2;
+        float tm2;
+        instance_ray(in, ro, rd, R1.tmax, &o2, &d2, &tm2);
+        trav_init(T2, R2, o2, d2, tm2, instance_bounds(in));
+        bn = a.nodes + (size_t)in.node_off * 4;
+        bb = a.tri_base + in.node_off;
+        bt = a.tris + (size_t)in.tri_off * 3;
+        cur_inst = k;
+        cur_tri_off = in.tri_off;
+        return true;
+    }
+    // one step; true when the walk is complete
+    __device__ bool step(const TraceArgs &a) {
+        TraceCounters ctr;
+        if (state == 2) {
+            if (!(T2.cur_y & 0xff000000u) || trav_step<ANY_HIT, false>(T2, R2, S2, bn, bb, bt, a.lut, &ctr, ALPHA::of(a).at(cur_tri_off))) {
+                overflow += (T2.sp & B200PT_SP_OVERFLOW) ? 1u : 0u;
+                T2.sp &= B200PT_SP_MASK;
+                state = 1;
+                if (R2.best != B200PT_MISS) {
+                    best = cur_tri_off + R2.best;
+                    inst = cur_inst;
+                    hit = R2.hit;
+                    R1.tmax = R2.hit.t;  // r.tMax = ray.tMax (primitive.cpp:91)
+                    trav_rescale(T1, R1, R1.tmax);
+                    if (ANY_HIT) state = 3;
+                }
+            }
+        } else if (state == 1) {
+            if (a.tlas_node_off == 0u) {
+                if (next_linear < a.n_instances) {
+                    if (enter(a, next_linear)) state = 2;
+                    ++next_linear;
+                } else {
+                    state = 3;
+                }
+            } else if (pend_y) {
+                const int j = msb32(pend_y);
+                pend_y &= ~(1u << j);
+                const F4 *tt = a.tris + (size_t)a.tlas_tri_off * 3;
+                const uint32_t k = __float_as_uint(ld_f4(tt + (size_t)(pend_x + (uint32_t)j) * 3).w);  // TriRecord::prim
+                if (enter(a, k)) state = 2;
+            } else {
+                state = 0;
+            }
+        } else if (state == 0) {
+            const U4 *tn = a.nodes + (size_t)a.tlas_node_off * 4;
+            const uint32_t *tb1 = a.tri_base + a.tlas_node_off;
+            if (T1.cur_y & 0xff000000u) {
+                uint32_t lg_x = 0, lg_y = 0;
+                trav_node_phase<!ANY_HIT, false>(T1, S1, tn, tb1, a.lut, &lg_x, &lg_y, &ctr);
+                leaf_group_triangles(tb1, lg_x, lg_y, &pend_x, &pend_y);
+                state = 1;
+            } else if (!trav_next_group(T1, S1)) {
+                state = 3;
+            }
+        }
+        if (state == 3) {
+            overflow += (T1.sp & B200PT_SP_OVERFLOW) ? 1u : 0u;
+            T1.sp &= B200PT_SP_MASK;
+            if (overflow && a.stats) atomicAdd(&a.stats[7], (unsigned long long)overflow);
+            overflow = 0;
+            return true;
+        }
+        return false;
+    }
+};
+
+// ---------------------------------------------------------------------- spheres + instances
+// Scene::Intersect / IntersectP for the Sphere shapes (not part of the BVH) and the object instances: the rays of
+// the traversal launch that just finished (tMax shortened by its triangle hit).  Persistent warps; a lane that finished
+// its ray takes the next one as soon as fewer than refill_lanes lanes of the warp are still walking (like k_trace).
+template <bool ANY_HIT, bool CLASSIFY, class ALPHA>
+__global__ void __launch_bounds__(128) k_spheres(const TraceArgs a) {
+    const uint32_t n = *a.count;
+#ifndef B200PT_HOST_EMU
+    const int lane = threadIdx.x & 31;
+#endif
+    InstanceWalk<ANY_HIT, ALPHA> W;
+    uint32_t slot = 0, best = B200PT_MISS;
+    bool has = false, fin = false, exhausted = false, occluded = false;
+    while (true) {
+        // ---- converged: retire finished rays
+        {
+            int family = -1;
+            if (fin) {
+                if (ANY_HIT) {
+                    if (occluded || W.best != B200PT_MISS) slot_out(a.occ_out, slot, a.out_stride) = 1;
+                } else {
+                    if (W.best != B200PT_MISS) {
+                        best = W.best;
+                        if (a.hit_out) slot_out(a.hit_out, slot, a.out_stride) = best;
+                        if (a.hit_inst_out) slot_out(a.hit_inst_out, slot, a.out_stride) = W.inst;
+                        if (a.full_out) {
+                            b200pt_hit r;
+                            r.triangle = (int32_t)__float_as_uint(ld_f4(a.tris + (size_t)best * 3).w);
+                            r.t = W.hit.t;
+                            r.b0 = W.hit.b0;
+                            r.b1 = W.hit.b1;
+                            a.full_out[slot] = r;
+                        }
+                    }
+                    if (CLASSIFY && best != B200PT_MISS) {
+                        const uint32_t mf = is_sphere_hit(best) ? a.spheres[best & SPHERE_HIT_MASK].mat_flags
+                                                                : __float_as_uint(ld_f4(a.tris + (size_t)best * 3 + 1).w);
+                        family = hit_family(a.materials, mf);
+                    }
+                }
+            }
+            if (CLASSIFY) append_family(a.q_mat, a.qcount_mat, family, slot);
+            fin = false;
+        }
+        // ---- converged: idle lanes fetch new rays, test the spheres, set up the walk over the instances.  warp_append
+        // written out (the check build's one-lane form below): through warp_append this kernel compiles to another
+        // schedule, and cfg5rgb's separate pass (B200PT_NO_TRACE2=1) took 1762 and 1762 ms per step against 1748 and
+        // 1748 written out (bench.py, the two builds alternating, H100 80GB HBM3 at 700 W)
+        {
+            const bool want = !has && !exhausted;
+            uint32_t i = 0;
+            bool got = false;
+#ifdef B200PT_HOST_EMU
+            if (want) {
+                i = atomicAdd(a.sphere_work, 1u);
+                got = i < n;
+                exhausted = !got;
+            }
+#else
+            const uint32_t mask = __ballot_sync(FULL_MASK, want);
+            if (mask) {
+                const int leader = __ffs(mask) - 1;
+                uint32_t base = 0;
+                if (lane == leader) base = atomicAdd(a.sphere_work, (uint32_t)__popc(mask));
+                base = __shfl_sync(FULL_MASK, base, leader);
+                if (want) {
+                    i = base + (uint32_t)__popc(mask & ((1u << lane) - 1u));
+                    got = i < n;
+                    exhausted = !got;
+                }
+            }
+#endif
+            if (got) {
+                slot = a.queue ? a.queue[i] : i;
+                const float4 o4 = a.ray_o[(size_t)slot * a.stride];
+                const float4 d4 = a.ray_d[(size_t)slot * a.stride];
+                const V3 ro = v3(o4), rd = v3(d4);
+                float tmax = a.t_max_from_w ? o4.w : a.fixed_t_max;
+                best = B200PT_MISS;
+                occluded = false;
+                if (ANY_HIT) {
+                    occluded = slot_out(a.occ_out, slot, a.out_stride) != 0;
+                    for (uint32_t k = 0; k < a.n_spheres && !occluded; ++k) {
+                        float t;
+                        if (sphere_leaf_test(a.spheres[k], ro, rd, tmax) && sphere_intersect(a.spheres[k], ro, rd, tmax, &t, nullptr)) {
+                            slot_out(a.occ_out, slot, a.out_stride) = 1;
+                            occluded = true;
+                        }
+                    }
+                } else {
+                    if (a.hit_out) {
+                        best = slot_out(a.hit_out, slot, a.out_stride);
+                        if (best != B200PT_MISS) {  // ray.tMax after the triangle hit: Triangle::Intersect's t
+                            const F4 *tp = a.tris + (size_t)best * 3;
+                            const F4 t0 = ld_f4(tp), t1 = ld_f4(tp + 1), t2 = ld_f4(tp + 2);
+                            V3 o2 = ro, d2 = rd;
+                            if ((__float_as_uint(t1.w) & B200PT_TRI_INSTANCED) && a.hit_inst_out) {
+                                // a triangle of an instanced object (found by the two-level kernel): the same ray parameter in
+                                // the object's space (primitive.cpp:91)
+                                float tm2;
+                                instance_ray(a.instances[slot_out(a.hit_inst_out, slot, a.out_stride)], ro, rd, pt_inf(), &o2, &d2, &tm2);
+                            }
+                            TriHit h;
+                            if (triangle_test(v3(t0), v3(t1), v3(t2), o2, make_shear(d2), pt_inf(), &h)) tmax = h.t;
+                        }
+                    } else if (a.full_out[slot].triangle >= 0) {
+                        tmax = a.full_out[slot].t;
+                        best = 0u;  // some top-level triangle (only its presence matters below: full_out keeps the record)
+                    }
+                    uint32_t sph = B200PT_MISS;
+                    for (uint32_t k = 0; k < a.n_spheres; ++k) {
+                        float t;
+                        if (sphere_leaf_test(a.spheres[k], ro, rd, tmax) && sphere_intersect(a.spheres[k], ro, rd, tmax, &t, nullptr)) {
+                            tmax = t;
+                            sph = k;
+                        }
+                    }
+                    if (sph != B200PT_MISS) {
+                        best = SPHERE_HIT_BASE | sph;
+                        if (a.hit_out) slot_out(a.hit_out, slot, a.out_stride) = best;
+                        if (a.full_out) {
+                            b200pt_hit r;
+                            r.triangle = (int32_t)(a.n_tris + sph);
+                            r.t = tmax;
+                            r.b0 = r.b1 = 0.f;
+                            a.full_out[slot] = r;
+                        }
+                    }
+                }
+                W.best = B200PT_MISS;
+                if (a.n_instances && !(ANY_HIT && occluded)) {
+                    W.init(a, ro, rd, tmax);
+                    has = true;
+                } else {
+                    fin = true;  // nothing to walk: retire in the next round
+                }
+            }
+        }
+#ifdef B200PT_HOST_EMU
+        while (has) {
+            if (W.step(a)) {
+                has = false;
+                fin = true;
+            }
+        }
+        if (!fin && exhausted) break;
+#else
+        if (__ballot_sync(FULL_MASK, has || fin) == 0) break;
+        while (has) {
+            if (W.step(a)) {
+                has = false;
+                fin = true;
+            }
+            if (__popc(__activemask()) < a.sphere_refill_lanes) break;
+        }
+        __syncwarp();
+#endif
+    }
 }
-#define B200PT_WALK(x) x
-#define B200PT_WALK_ALPHA(off)
-#include "spheres_kernel.cuh"
-#undef B200PT_WALK
-#undef B200PT_WALK_ALPHA
-#define B200PT_WALK(x) x##_alpha
-#define B200PT_WALK_ALPHA(off) , AlphaTest::of(a).at(off)
-#include "spheres_kernel.cuh"
-#undef B200PT_WALK
-#undef B200PT_WALK_ALPHA
 
 #endif  // B200PT_NSPEC == 3
 __device__ __forceinline__ DeltaLight delta_of(const DevLight &l, const Spec &intensity) {
@@ -2531,79 +3006,69 @@ void launch_raygen(const RenderDev *dev, uint32_t batch_first_tile, uint32_t n_b
 }
 
 #if B200PT_NSPEC == 3  // spectrum-independent: compiled once, in the RGBSpectrum translation unit
+template <class ALPHA>
+static void launch_trace_as(const TraceArgs &a, bool any_hit, bool classify, bool count, int grid, cudaStream_t s) {
+    if (any_hit) {
+        if (count)
+            B200PT_LAUNCH(B200PT_KERNEL(k_trace<true, false, true, ALPHA>), grid, 128, s, a);
+        else
+            B200PT_LAUNCH(B200PT_KERNEL(k_trace<true, false, false, ALPHA>), grid, 128, s, a);
+    } else if (classify) {
+        if (count)
+            B200PT_LAUNCH(B200PT_KERNEL(k_trace<false, true, true, ALPHA>), grid, 128, s, a);
+        else
+            B200PT_LAUNCH(B200PT_KERNEL(k_trace<false, true, false, ALPHA>), grid, 128, s, a);
+    } else {
+        if (count)
+            B200PT_LAUNCH(B200PT_KERNEL(k_trace<false, false, true, ALPHA>), grid, 128, s, a);
+        else
+            B200PT_LAUNCH(B200PT_KERNEL(k_trace<false, false, false, ALPHA>), grid, 128, s, a);
+    }
+}
 void launch_trace(const TraceArgs &a, bool any_hit, bool classify, bool count, int n_sm, cudaStream_t s) {
 #ifdef B200PT_HOST_EMU
     const int grid = n_sm;  // the per-ray k_trace of the check build has no occupancy to fill
 #else
     const int grid = n_sm * B200PT_TRACE_CTAS;
 #endif
-    if (a.alpha_masks) {
-        if (any_hit) {
-            if (count)
-                B200PT_LAUNCH(B200PT_KERNEL(k_trace_alpha<true, false, true>), grid, 128, s, a);
-            else
-                B200PT_LAUNCH(B200PT_KERNEL(k_trace_alpha<true, false, false>), grid, 128, s, a);
-        } else if (classify) {
-            if (count)
-                B200PT_LAUNCH(B200PT_KERNEL(k_trace_alpha<false, true, true>), grid, 128, s, a);
-            else
-                B200PT_LAUNCH(B200PT_KERNEL(k_trace_alpha<false, true, false>), grid, 128, s, a);
-        } else {
-            if (count)
-                B200PT_LAUNCH(B200PT_KERNEL(k_trace_alpha<false, false, true>), grid, 128, s, a);
-            else
-                B200PT_LAUNCH(B200PT_KERNEL(k_trace_alpha<false, false, false>), grid, 128, s, a);
-        }
-    } else if (any_hit) {
-        if (count)
-            B200PT_LAUNCH(B200PT_KERNEL(k_trace<true, false, true>), grid, 128, s, a);
-        else
-            B200PT_LAUNCH(B200PT_KERNEL(k_trace<true, false, false>), grid, 128, s, a);
-    } else if (classify) {
-        if (count)
-            B200PT_LAUNCH(B200PT_KERNEL(k_trace<false, true, true>), grid, 128, s, a);
-        else
-            B200PT_LAUNCH(B200PT_KERNEL(k_trace<false, true, false>), grid, 128, s, a);
-    } else {
-        if (count)
-            B200PT_LAUNCH(B200PT_KERNEL(k_trace<false, false, true>), grid, 128, s, a);
-        else
-            B200PT_LAUNCH(B200PT_KERNEL(k_trace<false, false, false>), grid, 128, s, a);
-    }
+    if (a.alpha_masks)
+        launch_trace_as<AlphaTest>(a, any_hit, classify, count, grid, s);
+    else
+        launch_trace_as<NoAlpha>(a, any_hit, classify, count, grid, s);
 }
 
 #ifndef B200PT_HOST_EMU
-void launch_trace2(const TraceArgs &a, bool any_hit, bool classify, int n_sm, cudaStream_t s) {
-    if (a.alpha_masks) {
-        if (any_hit)
-            B200PT_LAUNCH(B200PT_KERNEL(k_trace2_alpha<true, false>), n_sm * 6, 128, s, a);
-        else if (classify)
-            B200PT_LAUNCH(B200PT_KERNEL(k_trace2_alpha<false, true>), n_sm * 6, 128, s, a);
-        else
-            B200PT_LAUNCH(B200PT_KERNEL(k_trace2_alpha<false, false>), n_sm * 6, 128, s, a);
-    } else if (any_hit)
-        B200PT_LAUNCH(B200PT_KERNEL(k_trace2<true, false>), n_sm * 6, 128, s, a);
+template <class ALPHA>
+static void launch_trace2_as(const TraceArgs &a, bool any_hit, bool classify, int grid, cudaStream_t s) {
+    if (any_hit)
+        B200PT_LAUNCH(B200PT_KERNEL(k_trace2<true, false, ALPHA>), grid, 128, s, a);
     else if (classify)
-        B200PT_LAUNCH(B200PT_KERNEL(k_trace2<false, true>), n_sm * 6, 128, s, a);
+        B200PT_LAUNCH(B200PT_KERNEL(k_trace2<false, true, ALPHA>), grid, 128, s, a);
     else
-        B200PT_LAUNCH(B200PT_KERNEL(k_trace2<false, false>), n_sm * 6, 128, s, a);
+        B200PT_LAUNCH(B200PT_KERNEL(k_trace2<false, false, ALPHA>), grid, 128, s, a);
+}
+void launch_trace2(const TraceArgs &a, bool any_hit, bool classify, int n_sm, cudaStream_t s) {
+    if (a.alpha_masks)
+        launch_trace2_as<AlphaTest>(a, any_hit, classify, n_sm * 6, s);
+    else
+        launch_trace2_as<NoAlpha>(a, any_hit, classify, n_sm * 6, s);
 }
 #endif
 
-void launch_spheres(const TraceArgs &a, bool any_hit, bool classify, int grid, cudaStream_t s) {
-    if (a.alpha_masks) {
-        if (any_hit)
-            B200PT_LAUNCH(B200PT_KERNEL(k_spheres_alpha<true, false>), grid, 128, s, a);
-        else if (classify)
-            B200PT_LAUNCH(B200PT_KERNEL(k_spheres_alpha<false, true>), grid, 128, s, a);
-        else
-            B200PT_LAUNCH(B200PT_KERNEL(k_spheres_alpha<false, false>), grid, 128, s, a);
-    } else if (any_hit)
-        B200PT_LAUNCH(B200PT_KERNEL(k_spheres<true, false>), grid, 128, s, a);
+template <class ALPHA>
+static void launch_spheres_as(const TraceArgs &a, bool any_hit, bool classify, int grid, cudaStream_t s) {
+    if (any_hit)
+        B200PT_LAUNCH(B200PT_KERNEL(k_spheres<true, false, ALPHA>), grid, 128, s, a);
     else if (classify)
-        B200PT_LAUNCH(B200PT_KERNEL(k_spheres<false, true>), grid, 128, s, a);
+        B200PT_LAUNCH(B200PT_KERNEL(k_spheres<false, true, ALPHA>), grid, 128, s, a);
     else
-        B200PT_LAUNCH(B200PT_KERNEL(k_spheres<false, false>), grid, 128, s, a);
+        B200PT_LAUNCH(B200PT_KERNEL(k_spheres<false, false, ALPHA>), grid, 128, s, a);
+}
+void launch_spheres(const TraceArgs &a, bool any_hit, bool classify, int grid, cudaStream_t s) {
+    if (a.alpha_masks)
+        launch_spheres_as<AlphaTest>(a, any_hit, classify, grid, s);
+    else
+        launch_spheres_as<NoAlpha>(a, any_hit, classify, grid, s);
 }
 
 #endif  // B200PT_NSPEC == 3

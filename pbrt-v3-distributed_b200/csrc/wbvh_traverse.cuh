@@ -364,6 +364,10 @@ B200_HD void leaf_group_triangles(const uint32_t *__restrict__ tri_base, uint32_
 // Triangles without alpha masks: the watertight test alone decides.  Every scene without masks runs this.
 struct NoAlpha {
     static constexpr bool enabled = false;
+    template <class ARGS>
+    B200_HD static NoAlpha of(const ARGS &) {  // (a launch's arguments, as AlphaTest::of takes them)
+        return NoAlpha();
+    }
     B200_HD NoAlpha at(uint32_t) const { return *this; }
     B200_HD bool rejects(bool, uint32_t, uint32_t, uint32_t, const TriHit &) const { return false; }
 };
